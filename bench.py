@@ -1,14 +1,16 @@
 #!/usr/bin/env python
-"""bench.py -- Hi3D denoising hot path on B200.
+"""bench.py -- Hi3D denoising hot path on H100.
 
 One "step" = one orbital video of the workload: 25 Euler-EDM sampler steps of the CFG-batched VideoUNet
 (N = 2 x 16 frames) followed by the AutoencoderKL decode of the 16 frames.  Metric = multi-view frames / s.
 
 Default workload: BASELINE.json configs[2], second-stage 16 x 1024 x 1024 (latents 16 x 4 x 128 x 128, 17-channel UNet
 input = [x | depth 9 | cond latent 4], v02 re-noise loop), fp16 (the reference's inference dtype and the parity dtype;
-SURVEY F4) -- the largest single-GPU configuration and the shape the north-star target is stated on.  The stage-1 number
-(configs[1], 16 x 512 x 512) is measured in the same N=1 run and reported under the extra key `stage1`
-(`--stage 1` makes it the main line instead).
+SURVEY F4) -- the largest single-GPU configuration and the shape the north-star target is stated on.  `--with-stage1` adds the
+stage-1 number (16 x 512 x 512) of the same N=1 run under the extra key `stage1` (`--stage 1` makes it the main line
+instead).  The run times exactly --steps videos after exactly --warmup untimed ones; `e2e` adds the measured
+host-to-device copy of a video's inputs and device-to-host copy of its frames to the timed time per video, and `cpu_baseline` (one real reference sampler step on the host) is only taken with
+--cpu-baseline.
 With --gpus N > 1 (torchrun) the default is `--shard frames` (configs[3], the north-star layout): ONE video whose 16 frames
 are sharded over the ranks (strong scaling; K/V exchange before temporal attention, one-frame halo for the (3,1,1) convs,
 (sum, sumsq) exchange for the (T,H,W) GroupNorm -- through peer memory over NVLink inside the consuming kernels, or NCCL
@@ -17,12 +19,19 @@ In frames mode the line also carries `shard_selfcheck` (max |err| of one sharded
 unsharded on the same GPU) and `exchange` (device time of the separable exchange launches of one UNet forward).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--stage 1|2] [--shard videos|frames] [--impl reference]
+                    [--dump-outputs DIR]
+
+--dump-outputs DIR writes, after the timed steps, what the last timed video returned to its caller (the decoded frames,
+fp16 [16, 3, H, W]) as float32 .npy files: `frames_stride4.npy` = every 4th pixel in both directions of every frame and
+channel, `frames_sample.npy` = 2^22 elements of the flattened frames at indices drawn with torch.randint from a CPU
+generator seeded 20240901 (the same indices every run).  Inputs and synthetic weights are seeded, so two builds can be
+compared output for output.
 
 stdout carries exactly one line, the JSON (libraries that print to fd 1 are redirected to stderr).  Keys beyond the
 contract: `unet_ms_per_sampler_step` (one eager UNet forward with the host kept ahead of the GPU = the cost of a sampler
 step inside the graph), `kernel_breakdown` (CUDA events around every launch of one instrumented forward: per kernel class
 ms / share / TFLOP/s / GB/s, the top GEMM shapes, and the sum of launches), `roofline` (all GEMM launches of that forward
-against the measured sustained bf16 peak of MEASURED_PEAKS.json).
+against the sustained bf16 peak of MEASURED_PEAKS.json when present, else the H100 SXM data-sheet rate, labelled as such).
 
 --impl reference times THE REFERENCE ITSELF -- the unmodified `sgm` modules staged byte-for-byte under oracle/_ref by
 oracle/build_ref.py (kind "reference"; the oracle port only if that copy is absent) -- on the host cores, fp32, at the
@@ -55,7 +64,8 @@ def _peaks():
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], tf_burst=d["bf16_tflops"], tf_sust=d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                     src="measured")
-    return dict(hbm=6650.0, tf_burst=1590.0, tf_sust=1400.0, src="fallback")
+    # NVIDIA H100 SXM data sheet (dense fp16 / bf16, HBM3): a bound, not a measured rate
+    return dict(hbm=3350.0, tf_burst=989.0, tf_sust=989.0, src="H100 SXM data sheet")
 
 
 class ClockSampler:
@@ -135,19 +145,6 @@ def shard_frames(t: dict, rank: int, world: int) -> dict:
     return {k: (v[sl].contiguous() if v.shape[0] == T_FRAMES else v) for k, v in t.items()}
 
 
-# dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel, from the committed `ncu --set full` capture
-# (not measurable live): mean over the 10 hi3d_gemm_tc5 launches of input block 1 (64x64 level: conv3x3, temporal conv,
-# proj_in, qkv, attention out, GEGLU, ff2 ...), each 84-420 MB algorithmic.  Stage 2 was not captured.
-NCU_GEMM_TRAFFIC = {1: 292.8e6, 2: 1163.7e6}
-NCU_GEMM_TRAFFIC_NOTE = {
-    1: ("bytes per launch, mean of the 10 top-level GEMM launches in profiles/r01_ncu_full_stage1_final.txt "
-        "(ncu --set full, caches flushed per pass); `achieved` averages all 300 GEMM launches of a forward"),
-    2: ("dram__bytes_read.sum + dram__bytes_write.sum per launch, mean of the 13 top-level (128x128 latent) GEMM launches in "
-        "profiles/r02_ncu_full_stage2.txt (ncu --set full, caches flushed per pass; algorithmic bytes of the same launches: "
-        "A + output + residual = 0.67-1.7 GB); `achieved` averages all 300 GEMM launches of a forward"),
-}
-
-
 def kernel_breakdown(model, stage: int, dev_t, peaks):
     """One extra, instrumented sampler step: CUDA events around every launch of the UNet plan on the launching
     stream -> per kernel-class time, algorithmic FLOPs / bytes, achieved rate."""
@@ -211,9 +208,7 @@ def kernel_breakdown(model, stage: int, dev_t, peaks):
         ach = g["flops"] / g["ms"] / 1e9
         roof = dict(bound="tensor", kernel="hi3d_gemm (implicit-GEMM conv/linear, all launches of one UNet step)",
                     achieved=round(ach, 1), peak=peaks["tf_sust"], unit="TFLOP/s", frac=round(ach / peaks["tf_sust"], 4),
-                    peak_source=f"{peaks['src']} bf16_tflops_sustained", traffic=NCU_GEMM_TRAFFIC.get(stage),
-                    traffic_note=NCU_GEMM_TRAFFIC_NOTE.get(stage),
-                    flops_per_step=g["flops"], avg_launch_ms=round(g["ms"] / g["launches"], 4))
+                    peak_source=f"{peaks['src']} bf16_tflops_sustained", flops_per_step=g["flops"], avg_launch_ms=round(g["ms"] / g["launches"], 4))
     out["sum_of_launches_ms"] = round(tot, 3)
     return out, roof, fwd_ms
 
@@ -342,7 +337,21 @@ def unet_step_flops(stage: int, latent: int) -> float:
 
 
 # ------------------------------------------------------------------------------------------------------------------
-def measure(model, stage, engine, rank, world, local, dev, steps, warmup, frames_mode, dist, want_breakdown, peaks):
+def dump_outputs(out_dir: str, frames):
+    """--dump-outputs: the caller-visible result of the last timed video (see the module docstring)."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    f = frames.detach().float().cpu()
+    np.save(os.path.join(out_dir, "frames_stride4.npy"), f[:, :, ::4, ::4].contiguous().numpy())
+    flat = f.reshape(-1)
+    n = min(1 << 22, flat.numel())
+    idx = torch.randint(0, flat.numel(), (n,), generator=torch.Generator().manual_seed(20240901))
+    np.save(os.path.join(out_dir, "frames_sample.npy"), flat[idx].numpy())
+
+
+def measure(model, stage, engine, rank, world, local, dev, steps, warmup, frames_mode, dist, want_breakdown, peaks,
+            dump_dir=None):
     """Warm up, time `steps` videos device-resident and e2e; returns a dict of raw results (rank 0 has everything)."""
     import torch
     from hi3d_official_b200 import _native
@@ -376,24 +385,28 @@ def measure(model, stage, engine, rank, world, local, dev, steps, warmup, frames
             dist.all_reduce(ms, op=dist.ReduceOp.MAX)
         return float(ms.item()), _native.launch_count() - l0
 
+    last = {}
+
     def step_resident():
-        run_video(model, stage, dev_t, shard)
+        last["frames"] = run_video(model, stage, dev_t, shard)
 
-    def step_e2e():
+    def copies():
+        # a caller's host-device traffic per video: the inputs in, the decoded frames out
         d = {k: v.to(dev, non_blocking=True) for k, v in host.items()}
-        frames = run_video(model, stage, d, shard)
-        out_host.copy_(frames, non_blocking=True)
-        torch.cuda.current_stream().synchronize()
+        out_host.copy_(last["frames"], non_blocking=True)
+        return d
 
-    for _ in range(max(warmup, 3)):
+    for _ in range(warmup):
         step_resident()
     clocks = ClockSampler(local)
     if rank == 0:
         clocks.start()
     ms, launches = timed(step_resident, steps)
     clk = clocks.stop() if rank == 0 else None
-    step_e2e()
-    ms_e2e, _ = timed(step_e2e, steps)
+    if dump_dir and rank == 0 and not frames_mode:
+        dump_outputs(dump_dir, last["frames"])
+    copy_ms, _ = timed(copies, 1)
+    ms_e2e = ms / steps + copy_ms                  # one video with its copies
     res = dict(ms=ms, ms_e2e=ms_e2e, launches=launches, clocks=clk, h2d=h2d, d2h=d2h, breakdown=None, roof=None, unet_ms=None)
     if rank == 0 and want_breakdown and not frames_mode:
         res["breakdown"], res["roof"], res["unet_ms"] = kernel_breakdown(model, stage, dev_t, peaks)
@@ -510,7 +523,11 @@ def main():
                     help="latent size of the bounded cpu_baseline sample of the main arm (one real reference sampler step)")
     ap.add_argument("--ref-budget-s", type=float, default=float(os.environ.get("HI3D_REF_BUDGET_S", 300)),
                     help="--impl reference: wall-clock budget for the real full-size sampler steps")
-    ap.add_argument("--no-stage1", action="store_true", help="skip the extra stage-1 measurement of the N=1 stage-2 run")
+    ap.add_argument("--with-stage1", action="store_true", help="add a stage-1 measurement (key `stage1`) to an N=1 stage-2 run")
+    ap.add_argument("--cpu-baseline", action="store_true",
+                    help="add `cpu_baseline`: one real reference sampler step on the host cores (minutes of host time)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write samples of the last timed video's decoded frames as .npy files")
     ap.add_argument("--ref-latent", type=int, default=0,
                     help="TESTS ONLY (--impl reference): latent size override so the CPU suite finishes in seconds; the line "
                          "then says so in config.reference_latent_override and is not a bench value")
@@ -564,21 +581,21 @@ def main():
 
     model = build(args.stage)
     r = measure(model, args.stage, args.engine, rank, world, local, dev, args.steps, args.warmup, frames_mode, dist,
-                not args.no_breakdown, peaks)
+                not args.no_breakdown, peaks, dump_dir=args.dump_outputs)
     stage1 = None
-    if rank == 0 and world == 1 and args.stage == 2 and not args.no_stage1:
+    if rank == 0 and world == 1 and args.stage == 2 and args.with_stage1:
         del model
         torch.cuda.empty_cache()
-        k1 = max(1, min(args.steps, 5))
+        k1 = args.steps
         m1 = build(1)
-        r1 = measure(m1, 1, args.engine, 0, 1, local, dev, k1, 3, False, dist, not args.no_breakdown, peaks)
+        r1 = measure(m1, 1, args.engine, 0, 1, local, dev, k1, args.warmup, False, dist, not args.no_breakdown, peaks)
         stage1 = {"workload": workload(1)["name"], "value": T_FRAMES * k1 / (r1["ms"] / 1e3), "unit": "frames/s", "steps": k1,
-                  "warmup": 3, "ms_per_step": r1["ms"] / k1, "e2e": T_FRAMES * k1 / (r1["ms_e2e"] / 1e3),
+                  "warmup": args.warmup, "ms_per_step": r1["ms"] / k1, "e2e": T_FRAMES / (r1["ms_e2e"] / 1e3),
                   "unet_ms_per_sampler_step": r1["unet_ms"], "roofline": r1["roof"], "kernel_breakdown": r1["breakdown"]}
         del m1
         torch.cuda.empty_cache()
     cpu_b = None
-    if rank == 0 and world == 1 and not os.environ.get("HI3D_SKIP_CPU_BASELINE"):
+    if rank == 0 and world == 1 and args.cpu_baseline:
         lat = min(args.cpu_latent, wl["h"])
         threads = host_threads()
         ref = ReferenceCPU(args.stage, threads)
@@ -594,7 +611,7 @@ def main():
         videos = 1 if frames_mode else world
         ms, ms_e2e = r["ms"], r["ms_e2e"]
         fps = T_FRAMES * args.steps * videos / (ms / 1e3)
-        fps_e2e = T_FRAMES * args.steps * videos / (ms_e2e / 1e3)
+        fps_e2e = T_FRAMES * videos / (ms_e2e / 1e3)
         line = {"metric": METRIC, "value": fps, "unit": "frames/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
                 "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": "strong" if frames_mode else "weak",
                 "vs_baseline": None, "dtype": "fp16", "data": "synthetic", "config": config, "engine": args.engine,

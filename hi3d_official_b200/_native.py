@@ -2,7 +2,7 @@
 
 There is NO fallback: if the library cannot be loaded the import of any compute path raises, and every
 entry point raises `Hi3dError` on a non-zero return code.  The library is built in-tree by `build.py`
-(nvcc, sm_100a); on a box without nvcc the prebuilt .so that travelled with the snapshot is used.
+(nvcc, sm_90a); on a machine without nvcc an already built .so in the tree is used.
 """
 from __future__ import annotations
 
@@ -72,10 +72,9 @@ _SIGS = {
                                  C.c_void_p, C.c_float, C.c_void_p, C.c_void_p]),
     "hi3d_attention_d64": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_void_p]),
     "hi3d_attention_d64_tc5": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_void_p]),
-    "hi3d_attention_d512_tc5": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_void_p]),
     "hi3d_attention_tc5_set_exp_emulation": (C.c_int, [C.c_int]),
     "hi3d_attention_tc5_set_variant": (C.c_int, [C.c_int]),
-    "hi3d_attention_tc5_set_debug_buffer": (C.c_int, [C.c_void_p]),
+    "hi3d_attention_d512_tc5": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_void_p]),
     "hi3d_temporal_attention_d64": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
                                               C.c_void_p, C.c_void_p]),
     "hi3d_temporal_attention_d64_sharded": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int,

@@ -1,11 +1,13 @@
-"""Builds libhi3d_b200.so (the C-ABI CUDA library) in-tree with nvcc for sm_100a.
+"""Builds libhi3d_b200.so (the C-ABI CUDA library) in-tree with nvcc for the H100 (sm_90a).
 
-`nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo` per translation unit (parallel), then one
+`nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo` per translation unit (parallel), then one
 `nvcc -shared` link.  No torch headers are involved: the library is plain CUDA behind `include/hi3d_b200.h`
-and is loaded with ctypes (`_native.py`).  The .so is git-ignored but travels to the GPU box with the snapshot.
+and is loaded with ctypes (`_native.py`).  The .so, its digest stamp and the object files are build products
+(git-ignored).
 """
 from __future__ import annotations
 
+import hashlib
 import os
 import shutil
 import subprocess
@@ -16,10 +18,11 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 INC = os.path.join(os.path.dirname(HERE), "include")
 LIB = os.path.join(HERE, "libhi3d_b200.so")
+STAMP = LIB + ".sha256"                 # digest of what LIB was built from
 OBJ = os.path.join(HERE, "build")
 SOURCES = ["gemm_mma.cu", "gemm_tc5.cu", "attn.cu", "attn_tc5.cu", "norm.cu", "misc.cu", "peer.cu", "attn512_tc5.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo",
-              "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-I", INC]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = ARCH + ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-I", INC]
 
 
 def _nvcc() -> str:
@@ -29,13 +32,23 @@ def _nvcc() -> str:
     raise RuntimeError("nvcc not found; cannot build libhi3d_b200.so")
 
 
-def _deps_mtime() -> float:
-    files = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + [os.path.join(INC, "hi3d_b200.h"), __file__]
-    return max(os.path.getmtime(f) for f in files)
+def _digest() -> str:
+    """sha256 of every source, the public header and the compiler flags: the build identity of the library.  File times are
+    not used, so a built tree that is copied or checked out elsewhere (new times) is still recognised as built."""
+    h = hashlib.sha256(" ".join(ARCH + NVCC_FLAGS[len(ARCH):-2]).encode())
+    for f in sorted(os.listdir(CSRC)) + ["../../include/hi3d_b200.h"]:
+        h.update(f.encode())
+        with open(os.path.join(CSRC, f), "rb") as fh:
+            h.update(fh.read())
+    return h.hexdigest()
 
 
 def is_fresh() -> bool:
-    return os.path.exists(LIB) and os.path.getmtime(LIB) >= _deps_mtime()
+    try:
+        with open(STAMP) as f:
+            return os.path.exists(LIB) and f.read().strip() == _digest()
+    except OSError:
+        return False
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
@@ -43,15 +56,10 @@ def build(force: bool = False, verbose: bool = False) -> str:
         return LIB
     nvcc = _nvcc()
     os.makedirs(OBJ, exist_ok=True)
-    hdr_m = max(os.path.getmtime(os.path.join(CSRC, "common.cuh")), os.path.getmtime(os.path.join(CSRC, "tc5.cuh")), os.path.getmtime(os.path.join(INC, "hi3d_b200.h")),
-                os.path.getmtime(__file__))
 
     def cc(src):
-        s = os.path.join(CSRC, src)
         o = os.path.join(OBJ, src.replace(".cu", ".o"))
-        if not force and os.path.exists(o) and os.path.getmtime(o) >= max(os.path.getmtime(s), hdr_m):
-            return o
-        cmd = [nvcc] + NVCC_FLAGS + ["-c", s, "-o", o]
+        cmd = [nvcc] + NVCC_FLAGS + ["-c", os.path.join(CSRC, src), "-o", o]
         if verbose:
             cmd.insert(1, "-Xptxas=-v")
         r = subprocess.run(cmd, capture_output=True, text=True)
@@ -63,10 +71,12 @@ def build(force: bool = False, verbose: bool = False) -> str:
 
     with ThreadPoolExecutor(max_workers=min(8, len(SOURCES))) as ex:
         objs = list(ex.map(cc, SOURCES))
-    r = subprocess.run([nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB] + objs,
+    r = subprocess.run([nvcc, "-shared"] + ARCH + ["-o", LIB] + objs,
                        capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")
+    with open(STAMP, "w") as f:
+        f.write(_digest() + "\n")
     return LIB
 
 

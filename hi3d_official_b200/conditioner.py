@@ -9,7 +9,7 @@ that do not need third-party model weights, with the reference's names, ctor kwa
   AesEmbedder                           vtdm/encoders.py:56-90   ([score | timestep_embedding(100 score, 255)])
 
 The towers themselves -- OpenCLIP ViT-H (image embedding), MiDaS DPT-hybrid (depth), CLIP ViT-L + aesthetic MLP (score) --
-are third-party networks whose checkpoints are not available offline; they stay OUT of the B200 hot path (SURVEY §2).  Each
+are third-party networks whose checkpoints are not available offline; they stay OUT of the H100 hot path (SURVEY §2).  Each
 sits behind an `ExternalTower`: a callable installed with `.set_fn(...)`, or a pre-computed tensor passed in the batch under
 `<input_key>:<tower>` (e.g. batch["cond_frames_without_noise:clip"] = (B, 1024)).  Everything AROUND the towers is the
 reference's arithmetic, so the unmodified conditioner_config instantiates and, given tower outputs, produces the reference's
@@ -57,7 +57,7 @@ class ExternalTower(AbstractEmbModel):
     def forward(self, x):
         if self.fn is None:
             raise NotImplementedError(
-                f"{type(self).__name__}: this third-party tower (ctor kwargs {self.kwargs}) is outside the B200 hot path and its "
+                f"{type(self).__name__}: this third-party tower (ctor kwargs {self.kwargs}) is outside the H100 hot path and its "
                 f"checkpoint is not bundled; install it with .set_fn(callable) or pass its output in the batch "
                 f"(see hi3d_official_b200/conditioner.py)")
         return self.fn(x)

@@ -1,20 +1,14 @@
 // VAE mid-block attention (AttnBlock, model.py:180-201): ONE head of dimension 512 over L = (H/8)(W/8) tokens, as a
-// flash-attention kernel on tcgen05 / TMEM / TMA -- no L x L score matrix in memory, scores and softmax in fp32.
+// flash-attention kernel on Hopper (TMA + wgmma) -- no L x L score matrix in memory, scores and softmax in fp32.
 //
-// The head dimension does not fit the d = 64 kernel's layout: a 128 x 512 fp32 accumulator is all 512 TMEM columns, leaving
-// none for the scores.  So a CTA owns 128 queries and HALF of the value dimension (256 columns): grid (L/128, 2, images);
-// both halves compute the full S = Q K^T (contraction over 512) -- 1.5x the minimal tensor work, on a block that is ~1 % of
-// a video.  TMEM: S [0,128) fp32, P [128,192) packed fp16, O [192,448) fp32.
-//   S = sum over eight 64-wide chunks c of Q_c K_c^T: the 128 x 512 query tile (128 KB) stays RESIDENT in shared memory, the
-//       K chunks and the four 64-column V chunks of a key tile stream through one 4-stage ring of 16 KB tiles in the order
-//       the MMA warp consumes them (K(0) x8, V(0) x4, K(1) x8, ...): 192 KB from L2 per key tile and CTA.  (A first version
-//       re-fetched Q per key tile: 320 KB per tile, L2-bandwidth bound at ~3x the tensor time.)
-//   softmax: four warps, one thread per query row and 128 keys per tile in four 32-column sweeps, lazy reference maximum as
-//       in the d = 64 kernel (P <= 2^8; on overflow the row's accumulator is rescaled in TMEM and P redone from S, which P
-//       does not alias here),
-//   O += P V: four 64-column chunks of this CTA's half of V (MN-major B operand), A = P from TMEM.
-// The tensor pipe is the bound here (d = 512: 3072 MMA cycles per tile against 1024 MUFU cycles), issue order per tile:
-// P V(j), then S(j+1) -- P is single-buffered and must be consumed before the next softmax writes it.
+// A 64-query x 512 fp32 accumulator would be 256 registers per thread, so a CTA (one warpgroup) owns 64 queries and HALF of
+// the value dimension (256 columns): grid (L/64, 2, images); both halves compute the full S = Q K^T (contraction over
+// 512) -- 1.5x the minimal tensor work, on a block that is ~1 % of a video.
+//   S = sum over eight 64-wide chunks c of Q_c K_c^T: the 64 x 512 query tile (64 KB) stays RESIDENT in shared memory; the
+//       64 x 512 key tile (64 KB) and this CTA's 64 x 256 value half (32 KB) have one buffer each, refilled by TMA as soon as
+//       the MMAs that read them have retired (K(j+1) loads during softmax and P V(j), V(j+1) during S(j+1)).
+//   softmax: online, in registers (rows g and g + 8 of each warp's 16 rows per thread).
+//   O += P V: P from registers (the S accumulator fragment), V as four MN-major 64-column chunks.
 #include <cuda.h>
 #include <string.h>
 
@@ -23,238 +17,140 @@
 
 namespace hi3d {
 
-constexpr int F5_BM = 128, F5_BN = 128, F5_D = 512, F5_DV = 256;
-constexpr int F5_THREADS = 192;                    // warp 0 producer, warp 1 MMA, warps 2..5 softmax
-constexpr int F5_STAGES = 4;
-constexpr int F5_TILE = 128 * 128;                 // 128 rows x 64 fp16
-constexpr int F5_SMEM = 8 * F5_TILE + F5_STAGES * F5_TILE + 512 + 1024;
+constexpr int F5_BM = 64, F5_BN = 64, F5_D = 512, F5_DV = 256;
+constexpr int F5_THREADS = 128;
+constexpr int F5_TILE = 64 * 128;                  // 64 rows x 64 fp16
+constexpr int F5_SMEM = 8 * F5_TILE + 8 * F5_TILE + 4 * F5_TILE + 64 + 1024;
 
 struct Fa512Params {
-  CUtensorMap qkv_map;     // [rows, 1536] fp16 (q | k | v), box {64, 128}
+  CUtensorMap qkv_map;     // [rows, 1536] fp16 (q | k | v), box {64, 64}
   int L;
   float scale_log2;
   __half* out;             // [rows, 512]
 };
 
-HI3D_DEVINL float f5_ex2(float x) {
-  float r;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
-  return r;
-}
-
 __global__ void __launch_bounds__(F5_THREADS, 1) fmha512_tc5_kernel(const __grid_constant__ Fa512Params p) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
-  uint8_t* smem = smem_raw + (base - raw);
-  const uint32_t sQ = base;                                    // 8 chunks [128 queries x 64], resident
-  const uint32_t sR = base + 8 * F5_TILE;                      // ring: F5_STAGES tiles [128 keys x 64] (K chunks, then V chunks)
-  const uint32_t bar0 = sR + F5_STAGES * F5_TILE;
-  const uint32_t bar_full = bar0;                              // [STAGES]
-  const uint32_t bar_empty = bar0 + 8 * F5_STAGES;             // [STAGES]
-  const uint32_t bar_q = bar_empty + 8 * F5_STAGES;
-  const uint32_t bar_s_full = bar_q + 8;
-  const uint32_t bar_p_full = bar_s_full + 8;                  // 4 arrivals
-  const uint32_t bar_o_full = bar_p_full + 8;
-  const uint32_t tmem_slot = bar_o_full + 16;
-  volatile uint32_t* tmem_slot_g = reinterpret_cast<volatile uint32_t*>(smem + (tmem_slot - base));
+  const uint32_t sQ = base;                                    // 8 chunks [64 queries x 64], resident
+  const uint32_t sK = sQ + 8 * F5_TILE;                        // 8 chunks [64 keys x 64]
+  const uint32_t sV = sK + 8 * F5_TILE;                        // 4 chunks [64 keys x 64] of this CTA's value half
+  const uint32_t bar_q = sV + 4 * F5_TILE;
+  const uint32_t bar_k = bar_q + 8;
+  const uint32_t bar_v = bar_k + 8;
 
-  const int tid = threadIdx.x, lane = tid & 31;
-  const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int q0 = blockIdx.x * F5_BM;
   const int dvh = blockIdx.y;
   const int row0 = blockIdx.z * p.L;
   const int nkv = p.L / F5_BN;
 
-  if (warp == 0 && lane == 0) {
-    for (int s = 0; s < F5_STAGES; s++) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, 1); }
+  auto load_k = [&](int j) {
+    mbar_expect_tx(bar_k, 8 * F5_TILE);
+    for (int c = 0; c < 8; c++) tma_load_2d(sK + c * F5_TILE, &p.qkv_map, bar_k, F5_D + c * 64, row0 + j * F5_BN);
+  };
+  auto load_v = [&](int j) {
+    mbar_expect_tx(bar_v, 4 * F5_TILE);
+    for (int c = 0; c < 4; c++)
+      tma_load_2d(sV + c * F5_TILE, &p.qkv_map, bar_v, 2 * F5_D + dvh * F5_DV + c * 64, row0 + j * F5_BN);
+  };
+  if (tid == 0) {
     mbar_init(bar_q, 1);
-    mbar_init(bar_s_full, 1);
-    mbar_init(bar_p_full, 4);
-    mbar_init(bar_o_full, 1);
+    mbar_init(bar_k, 1);
+    mbar_init(bar_v, 1);
     asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
+    mbar_expect_tx(bar_q, 8 * F5_TILE);
+    for (int c = 0; c < 8; c++) tma_load_2d(sQ + c * F5_TILE, &p.qkv_map, bar_q, c * 64, row0 + q0);
+    load_k(0);
+    load_v(0);
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(tmem_slot), "r"(512));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_g;
-  const uint32_t tS0 = tmem_base, tP0 = tmem_base + 128, tO0 = tmem_base + 192;
 
-  if (warp == 0) {
-    // ======================= TMA producer =======================
-    if (elect_one()) {
-      mbar_expect_tx(bar_q, 8 * F5_TILE);
-      for (int c = 0; c < 8; c++) tma_load_2d(sQ + c * F5_TILE, &p.qkv_map, bar_q, c * 64, row0 + q0);
+  float o[4][32];
+#pragma unroll
+  for (int c = 0; c < 4; c++)
+#pragma unroll
+    for (int i = 0; i < 32; i++) o[c][i] = 0.f;
+  float mrow[2] = {-INFINITY, -INFINITY}, lrow[2] = {0.f, 0.f};
+  const float cl = p.scale_log2;
+  mbar_wait(bar_q, 0);
+
+  for (int j = 0; j < nkv; j++) {
+    // ---- S = sum_c Q_c K_c^T ----
+    mbar_wait(bar_k, j & 1);
+    float sc[32];
+    wgmma_fence();
+#pragma unroll
+    for (int c = 0; c < 8; c++) {
+      const uint64_t qd = gmma_desc_sw128(sQ + c * F5_TILE), kd = gmma_desc_sw128(sK + c * F5_TILE);
+#pragma unroll
+      for (int k = 0; k < 4; k++) wgmma_ss<64>(sc, qd + (uint64_t)(2 * k), kd + (uint64_t)(2 * k), (c | k) ? 1 : 0);
     }
-    __syncwarp();
-    uint32_t s = 0, ph = 0;
-    for (int j = 0; j < nkv; j++) {
-      for (int c = 0; c < 12; c++) {           // 8 K chunks, then this CTA's 4 V chunks
-        mbar_wait(bar_empty + 8 * s, ph ^ 1);
-        if (elect_one()) {
-          const uint32_t full = bar_full + 8 * s;
-          mbar_expect_tx(full, F5_TILE);
-          const int col = (c < 8) ? (F5_D + c * 64) : (2 * F5_D + dvh * F5_DV + (c - 8) * 64);
-          tma_load_2d(sR + s * F5_TILE, &p.qkv_map, full, col, row0 + j * F5_BN);
-        }
-        __syncwarp();
-        if (++s == F5_STAGES) { s = 0; ph ^= 1; }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(sc);
+    __syncthreads();                                           // every warp's MMAs on K(j) have retired
+    if (tid == 0 && j + 1 < nkv) load_k(j + 1);
+    // ---- online softmax ----
+    uint32_t pa[4][4];
+#pragma unroll
+    for (int hh = 0; hh < 2; hh++) {
+      float mx = -INFINITY;
+#pragma unroll
+      for (int nt = 0; nt < 8; nt++) mx = fmaxf(mx, fmaxf(sc[4 * nt + 2 * hh], sc[4 * nt + 2 * hh + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float mnew = fmaxf(mrow[hh], mx);
+      const float corr = exp2f((mrow[hh] - mnew) * cl);
+      const float moff = mnew * cl;
+      float rs = 0.f;
+#pragma unroll
+      for (int nt = 0; nt < 8; nt++) {
+        const float p0 = exp2f(sc[4 * nt + 2 * hh] * cl - moff);
+        const float p1 = exp2f(sc[4 * nt + 2 * hh + 1] * cl - moff);
+        rs += p0 + p1;
+        pa[nt >> 1][(nt & 1) * 2 + hh] = pack_half2(p0, p1);
       }
+      lrow[hh] = lrow[hh] * corr + rs;
+      mrow[hh] = mnew;
+#pragma unroll
+      for (int c = 0; c < 4; c++)
+#pragma unroll
+        for (int dt = 0; dt < 8; dt++) {
+          o[c][4 * dt + 2 * hh] *= corr;
+          o[c][4 * dt + 2 * hh + 1] *= corr;
+        }
     }
-  } else if (warp == 1) {
-    // ======================= MMA issuer =======================
-    const uint32_t idesc_qk = (1u << 4) | ((uint32_t)(F5_BN >> 3) << 17) | ((uint32_t)(F5_BM >> 4) << 24);
-    const uint32_t idesc_pv = (1u << 4) | (1u << 16) | ((uint32_t)(64 >> 3) << 17) | ((uint32_t)(F5_BM >> 4) << 24);
-    uint32_t s = 0, ph = 0;
-    auto issue_s = [&]() {     // S = sum_c Q_c K_c^T  (whole warp walks the ring, one elected lane issues)
-      for (int c = 0; c < F5_D / 64; c++) {
-        mbar_wait(bar_full + 8 * s, ph);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint64_t qd = umma_desc_sw128(sQ + c * F5_TILE), kd = umma_desc_sw128(sR + s * F5_TILE);
+    // ---- O += P V ----
+    mbar_wait(bar_v, j & 1);
+    wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < 4; k++) tc_mma_f16(tS0, qd + (uint64_t)(2 * k), kd + (uint64_t)(2 * k), idesc_qk, (c | k) ? 1u : 0u);
-          tc_commit(bar_empty + 8 * s);
-        }
-        __syncwarp();
-        if (++s == F5_STAGES) { s = 0; ph ^= 1; }
-      }
-      if (elect_one()) tc_commit(bar_s_full);
-      __syncwarp();
-    };
-    mbar_wait(bar_q, 0);
-    issue_s();
-    for (int j = 0; j < nkv; j++) {
-      mbar_wait(bar_p_full, j & 1);              // P(j) in TMEM, every softmax warp done with S(j)
-      for (int vc = 0; vc < 4; vc++) {
-        mbar_wait(bar_full + 8 * s, ph);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint64_t vd = umma_desc_sw128_mn(sR + s * F5_TILE);
+    for (int kk = 0; kk < 4; kk++)
 #pragma unroll
-          for (int k = 0; k < 8; k++)   // 16 keys per MMA: P advances 8 packed columns, V advances 16 rows (2048 B)
-            tc_mma_f16_ts(tO0 + 64u * vc, tP0 + (uint32_t)(8 * k), vd + (uint64_t)(128 * k), idesc_pv, (j | k) ? 1u : 0u);
-          tc_commit(bar_empty + 8 * s);
-          if (vc == 3) tc_commit(bar_o_full);
-        }
-        __syncwarp();
-        if (++s == F5_STAGES) { s = 0; ph ^= 1; }
-      }
-      if (j + 1 < nkv) issue_s();                // behind P V(j) on the tensor pipe: P(j) is consumed before softmax(j+1) starts
-    }
-  } else {
-    // ======================= softmax: one thread per query row =======================
-    const int q = warp & 3;                      // TMEM lane quarter of this warp (warps 2..5 -> quarters 2, 3, 0, 1)
-    const int r = q * 32 + lane;
-    const uint32_t lane_off = (uint32_t)(q * 32) << 16;
-    const float c = p.scale_log2;
-    const uint32_t tS = tS0 + lane_off, tP = tP0 + lane_off, tO = tO0 + lane_off;
-    float m_ref = -INFINITY, l_run = 0.f;
-    for (int j = 0; j < nkv; j++) {
-      mbar_wait(bar_s_full, j & 1);
-      tc_fence_after();
-      float tmax = m_ref, rsum = 0.f;
-      bool redo = (j == 0);
-      if (!redo) {
-        const float nmoff = -(m_ref * c);
-#pragma unroll 1
-        for (int cc = 0; cc < 4; cc++) {
-          uint32_t v[32];
-          tmem_ld32(tS + 32 * cc, v);
-          tmem_ld_wait(v);
-          uint32_t pk[16];
+      for (int c = 0; c < 4; c++) wgmma_rs_tb<64>(o[c], pa[kk], gmma_desc_sw128(sV + c * F5_TILE) + (uint64_t)(128 * kk), 1);
+    wgmma_commit();
+    wgmma_wait<0>();
 #pragma unroll
-          for (int i = 0; i < 32; i += 2) {
-            const float s0 = __uint_as_float(v[i]), s1 = __uint_as_float(v[i + 1]);
-            tmax = fmaxf(tmax, fmaxf(s0, s1));
-            const float p0 = f5_ex2(fmaf(s0, c, nmoff)), p1 = f5_ex2(fmaf(s1, c, nmoff));
-            rsum += p0 + p1;
-            pk[i >> 1] = pack_half2(p0, p1);
-          }
-          tmem_st16(tP + 16 * cc, pk);
-        }
-        redo = __any_sync(0xffffffffu, (tmax - m_ref) * c > 8.0f) != 0;
-        if (!redo) l_run += rsum;
-      }
-      if (redo) {
-        tmem_st_wait();
-        if (j == 0) {
-#pragma unroll 1
-          for (int cc = 0; cc < 4; cc++) {
-            uint32_t v[32];
-            tmem_ld32(tS + 32 * cc, v);
-            tmem_ld_wait(v);
-#pragma unroll
-            for (int i = 0; i < 32; i++) tmax = fmaxf(tmax, __uint_as_float(v[i]));
-          }
-        }
-        const float corr = f5_ex2((m_ref - tmax) * c);          // 0 on the first tile (m_ref = -inf)
-        m_ref = tmax;
-        if (j > 0) {
-          mbar_wait(bar_o_full, (j - 1) & 1);                   // O complete up to tile j-1 (normally long retired)
-          tc_fence_after();
-#pragma unroll 1
-          for (int cc = 0; cc < F5_DV / 16; cc++) {
-            uint32_t v[16];
-            tmem_ld16(tO + 16 * cc, v);
-            tmem_ld_wait16(v);
-#pragma unroll
-            for (int i = 0; i < 16; i++) v[i] = __float_as_uint(__uint_as_float(v[i]) * corr);
-            tmem_st16(tO + 16 * cc, v);
-          }
-        }
-        const float nmoff = -(tmax * c);
-        rsum = 0.f;
-#pragma unroll 1
-        for (int cc = 0; cc < 4; cc++) {
-          uint32_t v[32];
-          tmem_ld32(tS + 32 * cc, v);
-          tmem_ld_wait(v);
-          uint32_t pk[16];
-#pragma unroll
-          for (int i = 0; i < 32; i += 2) {
-            const float p0 = f5_ex2(fmaf(__uint_as_float(v[i]), c, nmoff)), p1 = f5_ex2(fmaf(__uint_as_float(v[i + 1]), c, nmoff));
-            rsum += p0 + p1;
-            pk[i >> 1] = pack_half2(p0, p1);
-          }
-          tmem_st16(tP + 16 * cc, pk);
-        }
-        l_run = l_run * corr + rsum;
-      }
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_p_full);
-    }
-    // ---- epilogue: O / l -> fp16, this CTA's 256 output columns of the row ----
-    mbar_wait(bar_o_full, (nkv - 1) & 1);
-    tc_fence_after();
-    const float inv = 1.f / l_run;
-    __half* dst = p.out + (long long)(row0 + q0 + r) * F5_D + dvh * F5_DV;
-#pragma unroll 1
-    for (int cc = 0; cc < F5_DV / 32; cc++) {
-      uint32_t v[32];
-      tmem_ld32(tO + 32 * cc, v);
-      tmem_ld_wait(v);
-#pragma unroll
-      for (int i = 0; i < 32; i += 8) {
-        Half8 o8;
-#pragma unroll
-        for (int k = 0; k < 4; k++)
-          o8.h[k] = __floats2half2_rn(__uint_as_float(v[i + 2 * k]) * inv, __uint_as_float(v[i + 2 * k + 1]) * inv);
-        *reinterpret_cast<Half8*>(dst + 32 * cc + i) = o8;
-      }
-    }
+    for (int c = 0; c < 4; c++) wgmma_fence_regs(o[c]);
+    __syncthreads();                                           // every warp's MMAs on V(j) have retired
+    if (tid == 0 && j + 1 < nkv) load_v(j + 1);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(tmem_base), "r"(512));
+
+  // ---- epilogue: O / l -> fp16, this CTA's 256 output columns of rows g and g + 8 ----
+  const int g = lane >> 2, t4 = lane & 3;
+#pragma unroll
+  for (int hh = 0; hh < 2; hh++) {
+    float l = lrow[hh];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    const float inv = 1.f / l;
+    __half* dst = p.out + (long long)(row0 + q0 + warp * 16 + g + 8 * hh) * F5_D + dvh * F5_DV + 2 * t4;
+#pragma unroll
+    for (int c = 0; c < 4; c++)
+#pragma unroll
+      for (int dt = 0; dt < 8; dt++)
+        *reinterpret_cast<uint32_t*>(dst + c * 64 + dt * 8) = pack_half2(o[c][4 * dt + 2 * hh] * inv, o[c][4 * dt + 2 * hh + 1] * inv);
   }
 }
 
@@ -263,7 +159,7 @@ __global__ void __launch_bounds__(F5_THREADS, 1) fmha512_tc5_kernel(const __grid
 using namespace hi3d;
 
 extern "C" int hi3d_attention_d512_tc5(const void* qkv, int n_img, int L, float scale, void* out, void* stream) {
-  if (!qkv || !out || n_img <= 0 || L <= 0 || (L % F5_BN) || n_img > 65535 || ((uintptr_t)qkv & 15) || ((uintptr_t)out & 15)) {
+  if (!qkv || !out || n_img <= 0 || L <= 0 || (L % 128) || n_img > 65535 || ((uintptr_t)qkv & 15) || ((uintptr_t)out & 15)) {
     set_error("hi3d_attention_d512_tc5: bad arguments (n_img=%d L=%d; L must be a multiple of 128)", n_img, L);
     return -2;
   }
@@ -272,7 +168,7 @@ extern "C" int hi3d_attention_d512_tc5(const void* qkv, int n_img, int L, float 
   {
     cuuint64_t dims[2] = {(cuuint64_t)(3 * F5_D), (cuuint64_t)n_img * (cuuint64_t)L};
     cuuint64_t str[1] = {(cuuint64_t)(3 * F5_D) * 2};
-    cuuint32_t box[2] = {64, 128};
+    cuuint32_t box[2] = {64, 64};
     if (encode_map(&fp.qkv_map, qkv, 2, dims, str, box, nullptr)) return -1;
   }
   fp.L = L;

@@ -1,44 +1,15 @@
-// Spatial self-attention core (head dim 64) on tcgen05 / TMEM / TMA.
+// Spatial self-attention core (head dim 64) on Hopper: TMA operand staging through an mbarrier ring and wgmma for both
+// products -- S = Q K^T with Q and K from shared memory, O += P V with P from registers (the S accumulator fragment is the
+// A-operand fragment of the next product, so P never touches shared memory) and V as an MN-major shared-memory operand.
 //
-// Two kernels live here.  The PRODUCTION kernel is fmha_tc5_split_kernel<EMU = 1, MODE = 2> further down (two independent
-// 64-key pipelines per CTA, register-lean softmax loop, a quarter of the exponentials on the FMA pipe, separate K / V
-// rings; 880 TFLOP/s at L = 16384).  fmha_tc5_kernel right below is its predecessor (eight softmax warps sharing one score
-// tile), kept selectable (hi3d_attention_tc5_set_variant(0)) because the measurements in DESIGN.md refer to it.  Its
-// description follows.
+// CTA = 128 queries x one (image, head), two warpgroups of 64 query rows; keys stream in tiles of BN (64 or 128) through a
+// ring of (K, V) tiles that both warpgroups read.  Thread 0 issues every TMA load; each warp releases a stage once its
+// warpgroup's MMAs on it have retired.  The key tail (L not a multiple of BN: keys of the next image or TMA out-of-bounds
+// zeros) is masked to -inf before the online softmax; query rows past L are computed and not stored.
 //
-// One CTA = 128 queries of one (image, head).  Per 128-key tile:
-//   S = Q K^T        tcgen05.mma, A = Q (smem, K-major), B = K tile (smem, K-major)      -> TMEM S[b]  (128 fp32 cols)
-//   softmax          4 warps, one thread per query row.  The kernel is bound by TMEM READ bandwidth (S is 64 KB per
-//                    tile), so S is normally read ONCE: P = exp2(S c - m_ref c) against the running maximum of the
-//                    previous tiles while the tile's own maximum is tracked in the same pass; only when some row of the
-//                    warp grew by more than 2^8 (or on the first tile) the warp falls back to max-then-exp (two reads)
-//                    and rescales.  P goes to its own 64 columns (packed fp16) so that S survives for the fallback.
-//   O  += P V        tcgen05.mma, A = P (TMEM), B = V tile (smem, MN-major: rows = keys), accumulating in TMEM O (64 fp32
-//                    cols).  Because the reference maximum only moves in the fallback path, O needs no per-tile
-//                    correction: it is rescaled in TMEM (ld, multiply, st by the row owner) only there.
-// 256 TMEM columns per CTA (S 128, P 64, O 64) and ~114 KB of shared memory, so TWO CTAs share an SM:
-// while one CTA's softmax warps work on a tile the other CTA's MMAs run, which keeps both the MUFU/FMA pipes and the
-// tensor pipe busy without splitting the softmax state across warpgroups.
-// Warp roles (320 threads): warp 0 = TMA producer (Q once, K/V ring), warp 1 = TMEM allocator + MMA issuer,
-// warps 2..9 = softmax: TWO warps per TMEM lane quarter, each owning 64 of the 128 key columns of its rows (the softmax
-// code is a latency-bound dependent chain per row -- profiled at ~0.2 IPC per warp with the softmax warps idle 40 % of the
-// time waiting for S -- so the rows are split across more warps rather than given more registers).  The two warps of a
-// quarter agree once per tile (a 64-thread named barrier) on whether the reference maximum has to move; the row sum is
-// kept per half and added at the end.
-//
-// Round-2 changes (profiles/r01_ncu_fmha_notes.txt: the softmax warps sat 24 % of their samples in the bar_s_full spin,
-// MUFU 52 % busy, tensor pipe 30 %):
-//   * S(j+1) = Q K(j+1)^T is issued BEFORE P(j) V(j): the S columns are dead once all softmax warps have signalled P(j),
-//     so the next tile's scores are computed while P V of this tile still waits its turn on the tensor pipe and the
-//     softmax warps start tile j+1 one MMA (~256 cycles) earlier.  P is single-buffered, so a warp waits for bar_o_full
-//     of tile j (P V(j) retired) before its FIRST tmem store of P(j+1) -- after it has loaded S and computed the first
-//     chunk of exponentials.
-//   * TMA producer / MMA issuer loops are whole-warp loops with elect.sync around the issue (uniform registers; the
-//     lane-0-only form cost 30 % in the GEMM, DESIGN.md lesson 1).
-//   * packed-fp32 softmax arithmetic (FFMA2 / FADD2): 6 issue slots per pair of scores instead of 9.
-//   * EMU > 0: a fraction (EMU / 4) of the exponentials is computed on the FMA pipe (Cody-Waite range reduction +
-//     cubic minimax polynomial, max relative error 7.5e-5, far below the fp16 rounding of P) to take load off the MUFU
-//     pipe, which bounds the kernel at 16384 ex2 per tile = 1024 cycles per tile-step and SM (FlashAttention-4's trick).
+// Variants (hi3d_attention_tc5_set_variant) choose the key tile and the ring depth; hi3d_attention_tc5_set_exp_emulation
+// moves a fraction (quarters, or 1/8, 3/8, 5/8) of the softmax exponentials from the MUFU pipe to the FMA pipe (exp2 by range reduction and a
+// cubic, relative error 1.6e-4 before the fp16 rounding of P).
 #include <cuda.h>
 #include <stdlib.h>
 #include <string.h>
@@ -48,904 +19,258 @@
 
 namespace hi3d {
 
-constexpr int FA_BM = 128;           // queries per CTA
-constexpr int FA_BN = 128;           // keys per tile
-constexpr int FA_STAGES = 2;         // K/V ring depth per CTA (two CTAs per SM -> 4 tiles in flight per SM)
-constexpr int FA_THREADS = 320;
-constexpr int FA_TILE_BYTES = 128 * 128;                 // 128 rows x 64 fp16
-constexpr int FA_XCH_BYTES = 4096;                       // per-quarter exchange: votes, partial maxima, partial sums
-constexpr int FA_SMEM = FA_TILE_BYTES * (1 + 2 * FA_STAGES) + 256 + FA_XCH_BYTES + 1024;
-
-HI3D_DEVINL float ex2_approx_ftz(float x) {
-  float r;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
-  return r;
-}
-
-// 2^x for a pair on the FMA pipe: n = round(x) through the 1.5 * 2^23 magic constant (the integer lands in the low mantissa
-// bits of t), f = x - n in [-0.5, 0.5], cubic minimax p(f) ~ 2^f (max relative error 7.5e-5), result = p * 2^n by adding
-// n << 23 to the exponent field.  x is clamped at -126 (2^-126 ~ 0 for a softmax weight); x <= 8 by the lazy-maximum rule.
-HI3D_DEVINL float2 ex2_emulated2(float2 x) {
-  const float MAGIC = 12582912.0f;
-  x.x = fmaxf(x.x, -126.0f);
-  x.y = fmaxf(x.y, -126.0f);
-  const float2 t = __fadd2_rn(x, make_float2(MAGIC, MAGIC));
-  const float2 n = __fadd2_rn(t, make_float2(-MAGIC, -MAGIC));
-  const float2 f = __fadd2_rn(x, make_float2(-n.x, -n.y));
-  float2 p = __ffma2_rn(make_float2(0.0551716648f, 0.0551716648f), f, make_float2(0.2426111251f, 0.2426111251f));
-  p = __ffma2_rn(p, f, make_float2(0.6932609677f, 0.6932609677f));
-  p = __ffma2_rn(p, f, make_float2(0.9999280572f, 0.9999280572f));
-  float2 r;
-  r.x = __int_as_float(__float_as_int(p.x) + (__float_as_int(t.x) << 23));
-  r.y = __int_as_float(__float_as_int(p.y) + (__float_as_int(t.y) << 23));
-  return r;
-}
-
-// P = 2^(s c - moff) for 32 scores of one row -> 16 packed half2; row sum into two packed-fp32 accumulators.
-template <int EMU>
-HI3D_DEVINL void softmax_exp32(const uint32_t (&cur)[32], float c, float nmoff, uint32_t (&pk)[16], float2 (&rs)[2]) {
-  const float2 c2 = make_float2(c, c), m2 = make_float2(nmoff, nmoff);
-#pragma unroll
-  for (int i = 0; i < 32; i += 2) {
-    const float2 x = __ffma2_rn(make_float2(__uint_as_float(cur[i]), __uint_as_float(cur[i + 1])), c2, m2);
-    float2 pe;
-    if (((i >> 1) & 3) < EMU) pe = ex2_emulated2(x);
-    else pe = make_float2(ex2_approx_ftz(x.x), ex2_approx_ftz(x.y));
-    rs[(i >> 1) & 1] = __fadd2_rn(rs[(i >> 1) & 1], pe);
-    pk[i >> 1] = pack_half2(pe.x, pe.y);
-  }
-}
-
-// The same for 16 scores -> 8 packed half2 at pk[OFF .. OFF + 8) (register-lean chunks of the split kernel's MODE 2 loop).
-// EMU8 = eighths of the exponentials on the FMA pipe (the emulated pairs are spread over the chunk).
-template <int EMU8, int OFF>
-HI3D_DEVINL void softmax_exp16(const uint32_t (&cur)[16], float c, float nmoff, uint32_t (&pk)[16], float2 (&rs)[2]) {
-  const float2 c2 = make_float2(c, c), m2 = make_float2(nmoff, nmoff);
-#pragma unroll
-  for (int i = 0; i < 16; i += 2) {
-    const float2 x = __ffma2_rn(make_float2(__uint_as_float(cur[i]), __uint_as_float(cur[i + 1])), c2, m2);
-    float2 pe;
-    if ((((i >> 1) * 5) & 7) < EMU8) pe = ex2_emulated2(x);
-    else pe = make_float2(ex2_approx_ftz(x.x), ex2_approx_ftz(x.y));
-    rs[(i >> 1) & 1] = __fadd2_rn(rs[(i >> 1) & 1], pe);
-    pk[OFF + (i >> 1)] = pack_half2(pe.x, pe.y);
-  }
-}
-HI3D_DEVINL void rowmax16(const uint32_t (&cur)[16], float (&mxa)[4]) {
-#pragma unroll
-  for (int i = 0; i < 16; i += 2)
-    mxa[(i >> 1) & 3] = fmaxf(mxa[(i >> 1) & 3], fmaxf(__uint_as_float(cur[i]), __uint_as_float(cur[i + 1])));
-}
+constexpr int FA_BM = 128;                 // queries per CTA
+constexpr int FA_MAX_STAGES = 5;
+constexpr int FA_THREADS = 256;
+constexpr int FA_QTILE = 64 * 128;         // 64 rows x 64 fp16
 
 struct FaParams {
-  CUtensorMap qkv_map;     // 2-D view of the packed [rows, 3C] matrix, box {64, 128}
-  int L, C, heads;
+  CUtensorMap q_map;       // [n_img * L, 3C] fp16 (q | k | v), box {64, 64}
+  CUtensorMap kv_map;      // the same matrix, box {64, BN}
+  int L, C, stages, emu8;   // emu8: eighths of the exponentials on the FMA pipe
   float scale_log2;
-  __half* out;
-  long long* dbg;          // MODE bit 3 (timeline instrumentation of CTA (0,0,0), tiles 16..23): [8 tiles][16 events] of clock64
+  __half* out;             // [n_img * L, C]
 };
 
-template <int EMU>
-__global__ void __launch_bounds__(FA_THREADS, 2) fmha_tc5_kernel(const __grid_constant__ FaParams p) {
+// (key tile, ring depth) of each variant.  Default: variant 6 without exponential emulation, the fastest on an H100 at the
+// benchmark's shapes (32 images x 5 heads, L = 16384: 290 TFLOP/s against 272 for (64, 3) and 225 for the 128-key tiles;
+// L = 4096: 288 against 280).
+constexpr int FA_NVARIANTS = 7;
+constexpr int FA_VARIANT_BN[FA_NVARIANTS] = {64, 64, 64, 128, 128, 128, 64};
+constexpr int FA_VARIANT_STAGES[FA_NVARIANTS] = {2, 4, 3, 2, 3, 4, 5};
+constexpr int FA_VARIANT_DEFAULT = 6;
+constexpr int FA_EMU_DEFAULT = 0;
+
+// 2^x for x <= 0 on the FMA pipe: x = j + f, 2^f by a cubic (relative error 1.6e-4), 2^j added to the exponent bits.
+HI3D_DEVINL float exp2_fma(float x) {
+  x = fmaxf(x, -127.f);
+  const float j = floorf(x);
+  const float f = x - j;
+  const float p = fmaf(fmaf(fmaf(0.07640766f, f, 0.22823162f), f, 0.6950504f), f, 1.0f);
+  return __int_as_float(__float_as_int(p) + ((int)j << 23));
+}
+
+template <int BN>
+__global__ void __launch_bounds__(FA_THREADS, 1) fmha_tc5_kernel(const __grid_constant__ FaParams p) {
+  constexpr int KV_TILE = BN * 128;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
   uint8_t* smem = smem_raw + (base - raw);
-  const uint32_t sQ = base;
-  const uint32_t sKV = base + FA_TILE_BYTES;                  // stage s: K at sKV + s*2T, V at + T
-  const uint32_t bar0 = base + FA_TILE_BYTES * (1 + 2 * FA_STAGES);
-  const uint32_t bar_q = bar0;                                // Q landed
-  const uint32_t bar_kv_full = bar0 + 8;                      // [STAGES]
-  const uint32_t bar_kv_empty = bar_kv_full + 8 * FA_STAGES;  // [STAGES]
-  const uint32_t bar_s_full = bar_kv_empty + 8 * FA_STAGES;   // S written by the MMA (phase flips every tile)
-  const uint32_t bar_p_full = bar_s_full + 16;                // P written by the softmax warps
-  const uint32_t bar_o_full = bar_p_full + 16;                // O written by the MMA (phase flips every tile)
-  const uint32_t tmem_slot = bar_o_full + 32;
-  volatile uint32_t* tmem_slot_g = reinterpret_cast<volatile uint32_t*>(smem + (tmem_slot - base));
+  const int STAGES = p.stages;
+  const uint32_t sQ = base;                                  // [128 queries x 64]
+  const uint32_t sR = base + 2 * FA_QTILE;                   // ring: STAGES x (K tile, V tile)
+  const uint32_t bar_q = sR + STAGES * 2 * KV_TILE;
+  const uint32_t bar_full = bar_q + 8;                       // [STAGES]
+  const uint32_t bar_empty = bar_full + 8 * FA_MAX_STAGES;   // [STAGES], one arrive per warp
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, lane = tid & 31;
+  const int cw = tid >> 7;                                   // warpgroup: query rows 64 cw .. + 63
+  const int warp = (tid >> 5) & 3;
   const int q0 = blockIdx.x * FA_BM;
   const int h = blockIdx.y;
-  const int row0 = blockIdx.z * p.L;          // first token row of this image
-  const int nkv = p.L / FA_BN;
+  const int row0 = blockIdx.z * p.L;
+  const int nkv = (p.L + BN - 1) / BN;
+  const int C = p.C;
 
-  if (warp == 0 && lane == 0) {
+  auto issue_kv = [&](int j, int s) {
+    const uint32_t full = bar_full + 8 * s;
+    mbar_expect_tx(full, 2 * KV_TILE);
+    tma_load_2d(sR + s * 2 * KV_TILE, &p.kv_map, full, C + h * 64, row0 + j * BN);
+    tma_load_2d(sR + s * 2 * KV_TILE + KV_TILE, &p.kv_map, full, 2 * C + h * 64, row0 + j * BN);
+  };
+  if (tid == 0) {
     mbar_init(bar_q, 1);
-    for (int s = 0; s < FA_STAGES; s++) { mbar_init(bar_kv_full + 8 * s, 1); mbar_init(bar_kv_empty + 8 * s, 1); }
-    mbar_init(bar_s_full, 1);
-    mbar_init(bar_p_full, 8);
-    mbar_init(bar_o_full, 1);
+    for (int s = 0; s < STAGES; s++) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, 8); }
     asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
+    mbar_expect_tx(bar_q, 2 * FA_QTILE);
+    tma_load_2d(sQ, &p.q_map, bar_q, h * 64, row0 + q0);
+    tma_load_2d(sQ + FA_QTILE, &p.q_map, bar_q, h * 64, row0 + q0 + 64);
+    for (int j = 0; j < STAGES && j < nkv; j++) issue_kv(j, j);
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(tmem_slot), "r"(256));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_g;
-  // TMEM columns: S = [0,128), P = [128,192) (packed fp16), O = [192,256)
-  const uint32_t tS0 = tmem_base, tP0 = tmem_base + 128, tO0 = tmem_base + 192;
 
-  if (warp == 0) {
-    // ======================= TMA producer: whole warp walks the loop, one elected lane issues =======================
-    if (elect_one()) {
-      mbar_expect_tx(bar_q, FA_TILE_BYTES);
-      tma_load_2d(sQ, &p.qkv_map, bar_q, h * 64, row0 + q0);
+  float o[32];
+#pragma unroll
+  for (int i = 0; i < 32; i++) o[i] = 0.f;
+  float mrow[2] = {-INFINITY, -INFINITY}, lrow[2] = {0.f, 0.f};
+  const int t4 = lane & 3;
+  const float c = p.scale_log2;
+  const uint64_t qd = gmma_desc_sw128(sQ + cw * FA_QTILE);
+  const int emu8 = p.emu8;
+  mbar_wait(bar_q, 0);
+
+  uint32_t s = 0, ph = 0;
+  for (int j = 0; j < nkv; j++) {
+    mbar_wait(bar_full + 8 * s, ph);
+    const uint32_t sK = sR + s * 2 * KV_TILE, sV = sK + KV_TILE;
+    // ---- S = Q K^T ----
+    float sc[BN / 2];
+    const uint64_t kd = gmma_desc_sw128(sK);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; k++) wgmma_ss<BN>(sc, qd + (uint64_t)(2 * k), kd + (uint64_t)(2 * k), k);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(sc);
+    // ---- mask the key tail ----
+    if ((j + 1) * BN > p.L) {
+#pragma unroll
+      for (int nt = 0; nt < BN / 8; nt++) {
+        const int col = j * BN + nt * 8 + 2 * t4;
+        if (col >= p.L) { sc[4 * nt] = -INFINITY; sc[4 * nt + 2] = -INFINITY; }
+        if (col + 1 >= p.L) { sc[4 * nt + 1] = -INFINITY; sc[4 * nt + 3] = -INFINITY; }
+      }
     }
+    // ---- online softmax: this thread holds rows g (hh = 0) and g + 8 (hh = 1) of its warp's 16 rows ----
+    uint32_t pa[BN / 16][4];
+#pragma unroll
+    for (int hh = 0; hh < 2; hh++) {
+      float mx = -INFINITY;
+#pragma unroll
+      for (int nt = 0; nt < BN / 8; nt++) mx = fmaxf(mx, fmaxf(sc[4 * nt + 2 * hh], sc[4 * nt + 2 * hh + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float mnew = fmaxf(mrow[hh], mx);
+      const float corr = exp2f((mrow[hh] - mnew) * c);
+      const float moff = mnew * c;
+      float rs = 0.f;
+#pragma unroll
+      for (int nt = 0; nt < BN / 8; nt++) {
+        const float x0 = sc[4 * nt + 2 * hh] * c - moff, x1 = sc[4 * nt + 2 * hh + 1] * c - moff;
+        const bool fma_pipe = (nt & 7) < emu8;       // emu8 eighths of the key columns
+        const float p0 = fma_pipe ? exp2_fma(x0) : exp2f(x0);
+        const float p1 = fma_pipe ? exp2_fma(x1) : exp2f(x1);
+        rs += p0 + p1;
+        // accumulator fragment -> A fragment: key columns 8 nt .. feed k16 step nt / 2, register (nt & 1) * 2 + hh
+        pa[nt >> 1][(nt & 1) * 2 + hh] = pack_half2(p0, p1);
+      }
+      lrow[hh] = lrow[hh] * corr + rs;
+      mrow[hh] = mnew;
+#pragma unroll
+      for (int dt = 0; dt < 8; dt++) {
+        o[4 * dt + 2 * hh] *= corr;
+        o[4 * dt + 2 * hh + 1] *= corr;
+      }
+    }
+    // ---- O += P V (16 keys per MMA: V advances 16 rows = 2048 bytes) ----
+    const uint64_t vd = gmma_desc_sw128(sV);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < BN / 16; kk++) wgmma_rs_tb<64>(o, pa[kk], vd + (uint64_t)(128 * kk), 1);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(o);
     __syncwarp();
-    for (int j = 0; j < nkv; j++) {
-      const int s = j % FA_STAGES;
-      mbar_wait(bar_kv_empty + 8 * s, ((j / FA_STAGES) & 1) ^ 1);
-      if (elect_one()) {
-        const uint32_t full = bar_kv_full + 8 * s;
-        mbar_expect_tx(full, 2 * FA_TILE_BYTES);
-        tma_load_2d(sKV + s * 2 * FA_TILE_BYTES, &p.qkv_map, full, p.C + h * 64, row0 + j * FA_BN);
-        tma_load_2d(sKV + s * 2 * FA_TILE_BYTES + FA_TILE_BYTES, &p.qkv_map, full, 2 * p.C + h * 64, row0 + j * FA_BN);
-      }
-      __syncwarp();
+    if (lane == 0) mbar_arrive(bar_empty + 8 * s);
+    if (tid == 0 && j + STAGES < nkv) {
+      mbar_wait(bar_empty + 8 * s, ph);          // both warpgroups are done with this stage
+      issue_kv(j + STAGES, s);
     }
-  } else if (warp == 1) {
-    // ======================= MMA issuer =======================
-    // S = Q K^T : M 128, N 128, A/B K-major.   O = P V : M 128, N 64, A from TMEM, B MN-major (bit 16).
-    const uint32_t idesc_qk = (1u << 4) | ((uint32_t)(FA_BN >> 3) << 17) | ((uint32_t)(FA_BM >> 4) << 24);
-    const uint32_t idesc_pv = (1u << 4) | (1u << 16) | ((uint32_t)(64 >> 3) << 17) | ((uint32_t)(FA_BM >> 4) << 24);
-    const uint64_t qd = umma_desc_sw128(sQ);
-    mbar_wait(bar_q, 0);
-    // prologue: S(0)
-    mbar_wait(bar_kv_full, 0);
-    tc_fence_after();
-    if (elect_one()) {
-      const uint64_t kd = umma_desc_sw128(sKV);
-#pragma unroll
-      for (int k = 0; k < 4; k++) tc_mma_f16(tS0, qd + (uint64_t)(2 * k), kd + (uint64_t)(2 * k), idesc_qk, k ? 1u : 0u);
-      tc_commit(bar_s_full);
-    }
-    __syncwarp();
-    for (int j = 0; j < nkv; j++) {
-      const int s = j % FA_STAGES;
-      mbar_wait(bar_p_full, j & 1);                           // P(j) is in TMEM; every softmax warp is done with S(j)
-      if (j + 1 < nkv) {
-        const int s1 = (j + 1) % FA_STAGES;
-        mbar_wait(bar_kv_full + 8 * s1, ((j + 1) / FA_STAGES) & 1);
-      }
-      tc_fence_after();
-      if (elect_one()) {
-        if (j + 1 < nkv) {                                    // S(j+1) first: the softmax warps start on it while P V(j) runs
-          const uint64_t kd = umma_desc_sw128(sKV + ((j + 1) % FA_STAGES) * 2 * FA_TILE_BYTES);
-#pragma unroll
-          for (int k = 0; k < 4; k++) tc_mma_f16(tS0, qd + (uint64_t)(2 * k), kd + (uint64_t)(2 * k), idesc_qk, k ? 1u : 0u);
-          tc_commit(bar_s_full);
-        }
-        const uint64_t vd = umma_desc_sw128_mn(sKV + s * 2 * FA_TILE_BYTES + FA_TILE_BYTES);
-#pragma unroll
-        for (int k = 0; k < 8; k++)   // 16 keys per MMA: P advances 8 packed columns, V advances 16 rows (2048 B)
-          tc_mma_f16_ts(tO0, tP0 + (uint32_t)(8 * k), vd + (uint64_t)(128 * k), idesc_pv, (j | k) ? 1u : 0u);
-        tc_commit(bar_o_full);
-        tc_commit(bar_kv_empty + 8 * s);
-      }
-      __syncwarp();
-    }
-  } else {
-    // ======================= softmax warps =======================
-    const int q = warp & 3;                      // TMEM lane quarter
-    const int hf = (warp - 2) >> 2;              // which half of the key columns of a tile this warp owns
-    const int r = q * 32 + lane;                 // query row within the tile == TMEM lane
-    const uint32_t lane_off = (uint32_t)(q * 32) << 16;
-    const float c = p.scale_log2;
-    // exchange area of this quarter: votes[2 tiles][2 halves], partial max / sum [2 tiles][2 halves][32 rows]
-    float* xch = reinterpret_cast<float*>(smem + (bar0 - base) + 256) + q * 256;
-    volatile int* votes = reinterpret_cast<volatile int*>(xch);             // [2][2]
-    volatile float* xmax = xch + 8;                                          // [2][2][32]
-    volatile float* xsum = xch + 8 + 128;                                    // [2][32]
-    const uint32_t tS = tS0 + lane_off + 64u * hf, tP = tP0 + lane_off + 32u * hf, tO = tO0 + lane_off + 32u * hf;
-    float m_run = -INFINITY, l_run = 0.f;        // l_run: sum over THIS warp's columns only
-    for (int j = 0; j < nkv; j++) {
-      mbar_wait(bar_s_full, j & 1);
-      tc_fence_after();
-      const int par = j & 1;
-      bool full = (j == 0);
-      if (!full) {
-        // ---- optimistic single read of S: exponentials against the running maximum, tile maximum on the side ----
-        const float nmoff = -(m_run * c);
-        float2 rs[2] = {make_float2(0.f, 0.f), make_float2(0.f, 0.f)};
-        float mxa[4] = {m_run, m_run, m_run, m_run};
-        uint32_t va[32], vb[32];
-        tmem_ld32(tS, va);
-        tmem_ld32(tS + 32, vb);
-#pragma unroll
-        for (int cc = 0; cc < 2; cc++) {
-          uint32_t (&cur)[32] = cc ? vb : va;
-          tmem_ld_wait(cur);
-#pragma unroll
-          for (int i = 0; i < 32; i += 2)
-            mxa[(i >> 1) & 3] = fmaxf(mxa[(i >> 1) & 3], fmaxf(__uint_as_float(cur[i]), __uint_as_float(cur[i + 1])));
-          uint32_t pk[16];
-          softmax_exp32<EMU>(cur, c, nmoff, pk, rs);
-          if (cc == 0) {                 // P is single-buffered: P V of the previous tile must have retired
-            mbar_wait(bar_o_full, (j - 1) & 1);
-            tc_fence_after();
-          }
-          tmem_st16(tP + 16 * cc, pk);
-        }
-        const float tmax = fmaxf(fmaxf(mxa[0], mxa[1]), fmaxf(mxa[2], mxa[3]));
-        // P <= 2^8 keeps fp16 exact enough and far from overflow; a larger jump redoes the tile with the true maximum.
-        // Both warps of the quarter must take the same path (they share the reference and the accumulator rows).
-        const int mine = __any_sync(0xffffffffu, (tmax - m_run) * c > 8.0f) ? 1 : 0;
-        if (lane == 0) votes[par * 2 + hf] = mine;
-        asm volatile("bar.sync %0, 64;\n" ::"r"(1 + q) : "memory");
-        full = (mine | votes[par * 2 + (hf ^ 1)]) != 0;
-        if (!full) l_run += (rs[0].x + rs[0].y) + (rs[1].x + rs[1].y);
-      }
-      if (full) {
-        // ---- max, then exponentials: two reads of S (first tile, or the maximum moved a lot) ----
-        tmem_st_wait();
-        float mxa[4] = {m_run, m_run, m_run, m_run};
-        {
-          uint32_t v0[32], v1[32];
-          tmem_ld32(tS, v0);
-          tmem_ld32(tS + 32, v1);
-          tmem_ld_wait(v0);
-#pragma unroll
-          for (int i = 0; i < 32; i++) mxa[i & 3] = fmaxf(mxa[i & 3], __uint_as_float(v0[i]));
-          tmem_ld_wait(v1);
-#pragma unroll
-          for (int i = 0; i < 32; i++) mxa[i & 3] = fmaxf(mxa[i & 3], __uint_as_float(v1[i]));
-        }
-        float mx = fmaxf(fmaxf(mxa[0], mxa[1]), fmaxf(mxa[2], mxa[3]));
-        xmax[(par * 2 + hf) * 32 + lane] = mx;
-        asm volatile("bar.sync %0, 64;\n" ::"r"(1 + q) : "memory");
-        mx = fmaxf(mx, xmax[(par * 2 + (hf ^ 1)) * 32 + lane]);
-        const float corr = exp2f((m_run - mx) * c);       // m_run = -inf on the first tile -> 0
-        const float moff = mx * c;
-        m_run = mx;
-        if (j > 0) {
-          // the reference moved: bring this warp's 32 accumulator columns (complete up to tile j-1) to the new one
-          mbar_wait(bar_o_full, (j - 1) & 1);
-          tc_fence_after();
-#pragma unroll 1
-          for (int cc = 0; cc < 2; cc++) {
-            uint32_t v[16];
-            tmem_ld16(tO + 16 * cc, v);
-            tmem_ld_wait16(v);
-#pragma unroll
-            for (int i = 0; i < 16; i++) v[i] = __float_as_uint(__uint_as_float(v[i]) * corr);
-            tmem_st16(tO + 16 * cc, v);
-          }
-          tmem_st_wait();
-        }
-        float2 rs[2] = {make_float2(0.f, 0.f), make_float2(0.f, 0.f)};
-        uint32_t va[32], vb[32];
-        tmem_ld32(tS, va);
-        tmem_ld32(tS + 32, vb);
-#pragma unroll
-        for (int cc = 0; cc < 2; cc++) {
-          uint32_t (&cur)[32] = cc ? vb : va;
-          tmem_ld_wait(cur);
-          uint32_t pk[16];
-          softmax_exp32<EMU>(cur, c, -moff, pk, rs);
-          tmem_st16(tP + 16 * cc, pk);
-        }
-        l_run = l_run * corr + (rs[0].x + rs[0].y) + (rs[1].x + rs[1].y);
-      }
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_p_full);
-    }
-    // row sum = both halves
-    xsum[hf * 32 + lane] = l_run;
-    asm volatile("bar.sync %0, 64;\n" ::"r"(1 + q) : "memory");
-    const float inv = 1.f / (l_run + xsum[(hf ^ 1) * 32 + lane]);
-    mbar_wait(bar_o_full, (nkv - 1) & 1);
-    tc_fence_after();
-    uint32_t v[32];
-    tmem_ld32(tO, v);
-    tmem_ld_wait(v);
-    __half* dst = p.out + (long long)(row0 + q0 + r) * p.C + h * 64 + 32 * hf;
-#pragma unroll
-    for (int i = 0; i < 32; i += 8) {
-      Half8 o8;
-#pragma unroll
-      for (int k = 0; k < 4; k++)
-        o8.h[k] = __floats2half2_rn(__uint_as_float(v[i + 2 * k]) * inv, __uint_as_float(v[i + 2 * k + 1]) * inv);
-      *reinterpret_cast<Half8*>(dst + i) = o8;
-    }
+    if (++s == (uint32_t)STAGES) { s = 0; ph ^= 1; }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(tmem_base), "r"(256));
+
+  // ---- finalize: O /= l, stage through this warpgroup's own Q rows, 16-byte stores ----
+  const int g = lane >> 2;
+  uint8_t* stage = smem + cw * FA_QTILE;
+#pragma unroll
+  for (int hh = 0; hh < 2; hh++) {
+    float l = lrow[hh];
+    l += __shfl_xor_sync(0xffffffffu, l, 1);
+    l += __shfl_xor_sync(0xffffffffu, l, 2);
+    const float inv = 1.f / l;
+    const int r = warp * 16 + g + 8 * hh;
+#pragma unroll
+    for (int dt = 0; dt < 8; dt++)
+      *reinterpret_cast<uint32_t*>(stage + swz128(r, dt) + t4 * 4) = pack_half2(o[4 * dt + 2 * hh] * inv, o[4 * dt + 2 * hh + 1] * inv);
+  }
+  __syncwarp();
+  __half* obase = p.out + (long long)row0 * C + h * 64;
+#pragma unroll
+  for (int i = 0; i < 4; i++) {
+    const int r = warp * 16 + (lane >> 3) + 4 * i;
+    const int ch = lane & 7;
+    const int q = q0 + cw * 64 + r;
+    if (q < p.L) {
+      const uint4 v = *reinterpret_cast<const uint4*>(stage + swz128(r, ch));
+      *reinterpret_cast<uint4*>(obase + (long long)q * C + ch * 8) = v;
+    }
   }
 }
 
-
-// =====================================================================================================================
-// Variant 2 ("split"): TWO INDEPENDENT HALF-TILE PIPELINES per CTA.
-//
-// Measured on the kernel above (ncu source sampling, profiles/r02_ncu_fmha_notes.txt): the softmax warps spend a third of
-// their samples waiting for S, because all eight of them share one S buffer, one reference maximum per row and one P
-// barrier -- the whole CTA moves in lock step through  S -> softmax -> P -> P V.  Here the 128 keys of a tile are two
-// halves of 64 with their OWN score columns, P columns, accumulator, barriers and row state:
-//   TMEM (256 columns): S_h = [64 h, 64 h + 64) fp32, P_h ALIASES the first 32 columns of S_h (packed fp16: the scores
-//   of a row live in the owning thread's registers once loaded, so the redo path needs no second TMEM read),
-//   O_h = [128 + 64 h, 192 + 64 h) fp32.
-//   A softmax thread owns one query row (TMEM lane) and the 64 keys of its half: its own reference maximum m_h, row sum
-//   l_h and the accumulator row of O_h.  No votes, no named barriers inside the loop; the two halves are merged once at
-//   the end: O = (O_a 2^((m_a - m) c) + O_b 2^((m_b - m) c)) / (l_a 2^(..) + l_b 2^(..)), m = max(m_a, m_b), through the
-//   (by then idle) K/V ring in shared memory.
-//   The MMA warp alternates between the halves: wait P_h(j) -> issue P_h V_h(j) (4 x N=64 MMAs) and S_h(j+1) (4 x N=64)
-//   -> commit.  In-order execution of the tensor pipe makes P_h V_h(j) read P before S_h(j+1) overwrites the aliased
-//   columns.  With two CTAs per SM this gives four pipelines per SM that drift out of phase, so the MUFU pipe (the bound:
-//   16384 ex2 per tile) always has a half-tile to work on.
-//   Each half-tile pipeline is a serial chain  S ready -> exponentials -> P announced -> MMA warp notices -> P V and next
-//   S issued -> S ready,  so the MMA warp's own latency per half is part of the period (tools/fmha_timeline.py): K and V
-//   have separate barriers (K is released one period before V), the operand barriers are passed BEFORE the wait for P and
-//   the loop is unrolled by the ring depth so that all descriptors are loop-invariant.
-// Template parameters (the production kernel is <EMU = 1, MODE = 2>; the others are kept for the record and the tests):
-//   EMU:        quarters of the exponentials evaluated on the FMA pipe (ex2_emulated2).
-//   MODE bit 0: the MMA warp serves whichever half has its P ready first (polls both barriers) instead of half 0, half 1.
-//   MODE bit 1: register-lean softmax loop -- the scores are read in four 16-column chunks and P is only stored once the
-//     whole half-tile has been accepted (row sum <= 2^12), so S stays intact in TMEM for the (rare) redo, which re-reads it
-//     in two passes; ~16 registers less at the peak, which is what lets the emulated exponentials fit without spilling.
-//   MODE bit 2: ping-pong turns between the two halves of a lane quarter (see the softmax loop).
-//   MODE bit 3: clock64 stamps of one CTA into FaParams::dbg (tools/fmha_timeline.py).
-//   MODE bit 4: the scores of a half arrive as two 32-key blocks, the first one issued AHEAD of P V (see serve_tile).
-// =====================================================================================================================
-template <int EMU, int MODE>
-__global__ void __launch_bounds__(FA_THREADS, 2) fmha_tc5_split_kernel(const __grid_constant__ FaParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw = smem_u32(smem_raw);
-  const uint32_t base = (raw + 1023u) & ~1023u;
-  uint8_t* smem = smem_raw + (base - raw);
-  const uint32_t sQ = base;
-  const uint32_t sKV = base + FA_TILE_BYTES;                  // stage s: K at sKV + s*2T, V at + T
-  const uint32_t bar0 = base + FA_TILE_BYTES * (1 + 2 * FA_STAGES);
-  const uint32_t bar_q = bar0;                                // Q landed
-  // K and V have their OWN full / empty barriers per stage: a K tile is free as soon as the S MMAs of both halves have
-  // read it (one tile period before the P V MMAs of the same tile retire), so its successor can be loaded a full period
-  // earlier than with one barrier per (K, V) pair -- clock stamps of the paired form showed the MMA warp waiting ~1000
-  // cycles per half-tile for K(j+1) (TMA latency ~1100 cycles against ~470 cycles of lookahead), 40 % of the tile period.
-  const uint32_t bar_k_full = bar0 + 8;                       // [STAGES]
-  const uint32_t bar_k_empty = bar_k_full + 8 * FA_STAGES;    // [STAGES]
-  const uint32_t bar_v_full = bar_k_empty + 8 * FA_STAGES;    // [STAGES]
-  const uint32_t bar_v_empty = bar_v_full + 8 * FA_STAGES;    // [STAGES]
-  const uint32_t bar_s_full = bar_v_empty + 8 * FA_STAGES;    // [2 halves]
-  const uint32_t bar_p_full = bar_s_full + 16;                // [2 halves], 4 arrivals each
-  const uint32_t bar_o_full = bar_p_full + 16;                // [2 halves]
-  const uint32_t bar_s2_full = bar_o_full + 16;               // [2 halves] (MODE bit 4: scores of the second 32 keys of a half)
-  const uint32_t tmem_slot = bar_s2_full + 32;
-  volatile uint32_t* tmem_slot_g = reinterpret_cast<volatile uint32_t*>(smem + (tmem_slot - base));
-
-  const int tid = threadIdx.x, lane = tid & 31;
-  const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
-  const int q0 = blockIdx.x * FA_BM;
-  const int h = blockIdx.y;
-  const int row0 = blockIdx.z * p.L;          // first token row of this image
-  const int nkv = p.L / FA_BN;
-
-  if (warp == 0 && lane == 0) {
-    mbar_init(bar_q, 1);
-    for (int s = 0; s < FA_STAGES; s++) {
-      mbar_init(bar_k_full + 8 * s, 1); mbar_init(bar_k_empty + 8 * s, 1);
-      mbar_init(bar_v_full + 8 * s, 1); mbar_init(bar_v_empty + 8 * s, 1);
-    }
-    for (int hh = 0; hh < 2; hh++) {
-      mbar_init(bar_s_full + 8 * hh, 1);
-      mbar_init(bar_p_full + 8 * hh, 4);
-      mbar_init(bar_o_full + 8 * hh, 1);
-      mbar_init(bar_s2_full + 8 * hh, 1);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
+static int g_variant = -1;   // -1 unread: HI3D_FMHA_VARIANT, else FA_VARIANT_DEFAULT
+static int g_emu = -1;       // -1 unread: HI3D_FMHA_EMU, else FA_EMU_DEFAULT
+static void read_env_once() {
+  if (g_variant < 0) {
+    const char* e = getenv("HI3D_FMHA_VARIANT");
+    g_variant = e ? atoi(e) : FA_VARIANT_DEFAULT;
+    if (g_variant < 0 || g_variant >= FA_NVARIANTS) g_variant = FA_VARIANT_DEFAULT;
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(tmem_slot), "r"(256));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n");
+  if (g_emu < 0) {
+    const char* e = getenv("HI3D_FMHA_EMU");
+    g_emu = e ? atoi(e) : FA_EMU_DEFAULT;
+    if (g_emu < 0 || g_emu > 7) g_emu = FA_EMU_DEFAULT;
   }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_g;
-  const uint32_t tS0 = tmem_base, tO0 = tmem_base + 128;      // S_h = tS0 + 64 h (P_h aliases its first 32 columns)
-  const bool dbg_cta = (MODE & 8) && p.dbg != nullptr && blockIdx.x == 1 && blockIdx.y == 0 && blockIdx.z == 0;
-#define FA_STAMP(J, E)                                                                     \
-  do {                                                                                     \
-    if constexpr (MODE & 8) {                                                              \
-      if (dbg_cta && lane == 0 && (J) >= 16 && (J) < 24) p.dbg[((J)-16) * 16 + (E)] = clock64(); \
-    }                                                                                      \
-  } while (0)
+}
 
-  if (warp == 0) {
-    // ======================= TMA producer =======================
-    if (elect_one()) {
-      mbar_expect_tx(bar_q, FA_TILE_BYTES);
-      tma_load_2d(sQ, &p.qkv_map, bar_q, h * 64, row0 + q0);
-    }
-    __syncwarp();
-    for (int j = 0; j < nkv; j++) {
-      const int s = j % FA_STAGES;
-      const uint32_t ph = ((j / FA_STAGES) & 1) ^ 1;
-      mbar_wait(bar_k_empty + 8 * s, ph);
-      if (elect_one()) {
-        mbar_expect_tx(bar_k_full + 8 * s, FA_TILE_BYTES);
-        tma_load_2d(sKV + s * 2 * FA_TILE_BYTES, &p.qkv_map, bar_k_full + 8 * s, p.C + h * 64, row0 + j * FA_BN);
-      }
-      __syncwarp();
-      mbar_wait(bar_v_empty + 8 * s, ph);
-      if (elect_one()) {
-        mbar_expect_tx(bar_v_full + 8 * s, FA_TILE_BYTES);
-        tma_load_2d(sKV + s * 2 * FA_TILE_BYTES + FA_TILE_BYTES, &p.qkv_map, bar_v_full + 8 * s, 2 * p.C + h * 64, row0 + j * FA_BN);
-      }
-      __syncwarp();
-    }
-  } else if (warp == 1) {
-    // ======================= MMA issuer =======================
-    // S_h = Q K_h^T : M 128, N 64, A/B K-major.   O_h += P_h V_h : M 128, N 64, A from TMEM, B MN-major (bit 16).
-    const uint32_t idesc_qk = (1u << 4) | ((uint32_t)(64 >> 3) << 17) | ((uint32_t)(FA_BM >> 4) << 24);
-    const uint32_t idesc_pv = (1u << 4) | (1u << 16) | ((uint32_t)(64 >> 3) << 17) | ((uint32_t)(FA_BM >> 4) << 24);
-    const uint32_t idesc_qk32 = (1u << 4) | ((uint32_t)(32 >> 3) << 17) | ((uint32_t)(FA_BM >> 4) << 24);   // N = 32
-    const uint64_t qd = umma_desc_sw128(sQ);
-    mbar_wait(bar_q, 0);
-    mbar_wait(bar_k_full, 0);
-    tc_fence_after();
-    if (elect_one()) {
-#pragma unroll
-      for (int hh = 0; hh < 2; hh++) {
-        // keys 64 hh .. 64 hh + 63 of the K tile: 8 swizzle row groups of 1024 bytes further on
-        const uint64_t kd = umma_desc_sw128(sKV + hh * 8192);
-        if constexpr (MODE & 16) {
-          // two N = 32 score blocks per half with their own barriers (see serve_tile)
-#pragma unroll
-          for (int k = 0; k < 4; k++) tc_mma_f16(tS0 + 64u * hh, qd + (uint64_t)(2 * k), kd + (uint64_t)(2 * k), idesc_qk32, k ? 1u : 0u);
-          tc_commit(bar_s_full + 8 * hh);
-#pragma unroll
-          for (int k = 0; k < 4; k++) tc_mma_f16(tS0 + 64u * hh + 32u, qd + (uint64_t)(2 * k), kd + (uint64_t)(256 + 2 * k), idesc_qk32, k ? 1u : 0u);
-          tc_commit(bar_s2_full + 8 * hh);
-        } else {
-#pragma unroll
-          for (int k = 0; k < 4; k++) tc_mma_f16(tS0 + 64u * hh, qd + (uint64_t)(2 * k), kd + (uint64_t)(2 * k), idesc_qk, k ? 1u : 0u);
-          tc_commit(bar_s_full + 8 * hh);
-        }
-      }
-      tc_commit(bar_k_empty);                                   // K(0) is free once both S(0) have been computed
-    }
-    __syncwarp();
-    // The per-half critical path  P announced -> P V and next S issued  is the kernel's period limiter (clock stamps: 186 +
-    // 349 + 410 cycles of this warp's own latency per half-tile against 256 cycles of tensor work), so everything that does
-    // not depend on P is done before the wait for it: the operand barriers of the tile (V(j), K(j+1) landed long ago) and
-    // the shared-memory descriptors (stage index static: the loop is unrolled by the ring depth).
-    uint64_t kdesc[FA_STAGES][2], vdesc[FA_STAGES][2];
-#pragma unroll
-    for (int s = 0; s < FA_STAGES; s++)
-#pragma unroll
-      for (int hh = 0; hh < 2; hh++) {
-        kdesc[s][hh] = umma_desc_sw128(sKV + s * 2 * FA_TILE_BYTES + hh * 8192);
-        vdesc[s][hh] = umma_desc_sw128_mn(sKV + s * 2 * FA_TILE_BYTES + FA_TILE_BYTES + hh * 8192);
-      }
-    auto serve_tile = [&](const int j, const int s, const int s1) {
-      const bool more = j + 1 < nkv;
-      mbar_wait(bar_v_full + 8 * s, (j / FA_STAGES) & 1);
-      if (more) mbar_wait(bar_k_full + 8 * s1, ((j + 1) / FA_STAGES) & 1);
-      uint32_t pend = 3u;                                       // halves of tile j not yet served (warp-uniform)
-      uint32_t polls = 0;
-      while (pend) {
-        int hh;
-        if constexpr (MODE & 1) {
-          // whichever half is ready: every lane must have seen the phase complete itself (uniform decision)
-          const bool r0 = (pend & 1u) && __all_sync(0xffffffffu, mbar_test(bar_p_full, j & 1));
-          const bool r1 = !r0 && (pend & 2u) && __all_sync(0xffffffffu, mbar_test(bar_p_full + 8, j & 1));
-          if (!r0 && !r1) {
-            if ((++polls & 0xfffffu) == 0u) mbar_wait(bar_p_full + ((pend & 1u) ? 0 : 8), j & 1);   // falls into the watchdog wait
-            continue;
-          }
-          hh = r0 ? 0 : 1;
-        } else {
-          hh = (pend & 1u) ? 0 : 1;
-          mbar_wait(bar_p_full + 8 * hh, j & 1);                // P_h(j) is in TMEM (aliasing S_h)
-        }
-        pend &= ~(1u << hh);
-        FA_STAMP(j, 6 + 3 * hh);
-        tc_fence_after();
-        FA_STAMP(j, 7 + 3 * hh);
-        if (elect_one()) {
-          const uint64_t vd = hh ? vdesc[s][1] : vdesc[s][0];
-          const uint64_t kd = hh ? kdesc[s1][1] : kdesc[s1][0];
-          if constexpr (MODE & 16) {
-            // MODE bit 4: the 64 score columns of a half are two 32-column blocks that swap roles every tile.  P(j) sits in
-            // block X = 32 (j & 1) (where the scores of the half's first 32 keys were); the other block Y was read completely
-            // before P was announced, so the scores of the first 32 keys of tile j+1 go there IMMEDIATELY -- ahead of P V(j) --
-            // and the softmax warps can start tile j+1 one P V + half an S earlier; the second 32 keys follow behind P V(j)
-            // into block X.  Three commits per half-tile: s_full (first block), o_full, s2_full (second block).
-            const uint32_t X = 32u * (uint32_t)s, Y = 32u - X;
-            if (more) {
-#pragma unroll
-              for (int k = 0; k < 4; k++) tc_mma_f16(tS0 + 64u * hh + Y, qd + (uint64_t)(2 * k), kd + (uint64_t)(2 * k), idesc_qk32, k ? 1u : 0u);
-              tc_commit(bar_s_full + 8 * hh);
-            }
-#pragma unroll
-            for (int k = 0; k < 4; k++)
-              tc_mma_f16_ts(tO0 + 64u * hh, tS0 + 64u * hh + X + (uint32_t)(8 * k), vd + (uint64_t)(128 * k), idesc_pv, (j | k) ? 1u : 0u);
-            tc_commit(bar_o_full + 8 * hh);
-            if (pend == 0u) tc_commit(bar_v_empty + 8 * s);
-            if (more) {
-#pragma unroll
-              for (int k = 0; k < 4; k++)   // keys 32 .. 63 of the half: 4 swizzle row groups (4096 B) further on
-                tc_mma_f16(tS0 + 64u * hh + X, qd + (uint64_t)(2 * k), kd + (uint64_t)(256 + 2 * k), idesc_qk32, k ? 1u : 0u);
-              tc_commit(bar_s2_full + 8 * hh);
-              if (pend == 0u) tc_commit(bar_k_empty + 8 * s1);
-            }
-          } else {
-#pragma unroll
-          for (int k = 0; k < 4; k++)   // 16 keys per MMA: P advances 8 packed columns, V advances 16 rows (2048 B)
-            tc_mma_f16_ts(tO0 + 64u * hh, tS0 + 64u * hh + (uint32_t)(8 * k), vd + (uint64_t)(128 * k), idesc_pv, (j | k) ? 1u : 0u);
-          tc_commit(bar_o_full + 8 * hh);
-          if (pend == 0u) tc_commit(bar_v_empty + 8 * s);       // both halves' P V of tile j have been issued
-          if (more) {                                           // in order behind P_h V_h(j): overwrites the aliased columns
-#pragma unroll
-            for (int k = 0; k < 4; k++) tc_mma_f16(tS0 + 64u * hh, qd + (uint64_t)(2 * k), kd + (uint64_t)(2 * k), idesc_qk, k ? 1u : 0u);
-            tc_commit(bar_s_full + 8 * hh);
-            if (pend == 0u) tc_commit(bar_k_empty + 8 * s1);    // both halves' S of tile j+1 have been issued
-          }
-          }
-        }
-        __syncwarp();
-        FA_STAMP(j, 8 + 3 * hh);
-      }
-    };
-    static_assert(FA_STAGES == 2, "the MMA loop is unrolled by the ring depth");
-    for (int j = 0; j < nkv; j += 2) {
-      serve_tile(j, 0, 1);
-      if (j + 1 < nkv) serve_tile(j + 1, 1, 0);
-    }
-  } else {
-    // ======================= softmax warps: (lane quarter q, key half hf) =======================
-    const int q = warp & 3;
-    const int hf = (warp - 2) >> 2;
-    const int r = q * 32 + lane;                 // query row within the tile == TMEM lane
-    const uint32_t lane_off = (uint32_t)(q * 32) << 16;
-    const float c = p.scale_log2;
-    const uint32_t tS = tS0 + lane_off + 64u * hf, tO = tO0 + lane_off + 64u * hf;
-    const uint32_t b_s = bar_s_full + 8 * hf, b_p = bar_p_full + 8 * hf, b_o = bar_o_full + 8 * hf;
-    float m_ref = -INFINITY, l_run = 0.f;        // reference maximum and row sum of THIS half
-    if constexpr (MODE & 2) {
-      // EMU 0 .. 4 = quarters; 5, 6, 7 = 3/8, 1/8, 5/8 (finer steps around the optimum, lean loop only)
-      constexpr int EMU8 = EMU <= 4 ? 2 * EMU : (EMU == 5 ? 3 : (EMU == 6 ? 1 : 5));
-      // MODE bit 2, ping-pong: the two warps of a lane quarter (halves 0 and 1 of this CTA; they share an SM sub-partition
-      // and its MUFU unit) take strict turns in their exponential phase through a pair of 64-thread named barriers.  Without
-      // it the four half-tile pipelines of an SM drift into a convoy: all of them in the exponential phase at once, sharing
-      // the MUFU pipe, then all of them waiting for their MMAs at once (ncu: 40 % of the softmax warps' samples in the
-      // bar_s_full wait while the XU pipe is 68 % busy).  With turns, one half computes while the other half's P V and next
-      // S run on the tensor pipe.
-      const int pp_mine = (hf == 0 ? 5 : 9) + q, pp_other = (hf == 0 ? 9 : 5) + q;
-      if constexpr (MODE & 4) {
-        if (hf == 1) asm volatile("bar.arrive %0, 64;\n" ::"r"(pp_other) : "memory");      // half 0 goes first
-      }
-      const uint32_t b_s2 = bar_s2_full + 8 * hf;
-      for (int j = 0; j < nkv; j++) {
-        mbar_wait(b_s, j & 1);
-        tc_fence_after();
-        if (q == 0) FA_STAMP(j, 3 * hf);
-        // block X holds the scores of the half's first 32 keys and later P; block Y the second 32 keys (MODE bit 4: the blocks
-        // swap roles every tile and Y is only valid after its own barrier; otherwise X = 0, Y = 32)
-        const uint32_t tX = (MODE & 16) ? tS + 32u * (uint32_t)(j & 1) : tS;
-        const uint32_t tY = (MODE & 16) ? tS + 32u - 32u * (uint32_t)(j & 1) : tS + 32u;
-        uint32_t a[16], b[16], pka[16], pkb[16];
-        float2 rs[2] = {make_float2(0.f, 0.f), make_float2(0.f, 0.f)};
-        bool redo = (j == 0);
-        if (redo) {
-          if constexpr (MODE & 4) asm volatile("bar.sync %0, 64;\n" ::"r"(pp_mine) : "memory");
-        } else {
-          // optimistic pass against the current reference; nothing is stored until the half-tile has been accepted
-          const float nmoff = -(m_ref * c);
-          tmem_ld16(tX, a);
-          if constexpr (MODE & 4) asm volatile("bar.sync %0, 64;\n" ::"r"(pp_mine) : "memory");   // my turn
-          tmem_ld_wait16(a);
-          tmem_ld16(tX + 16, b);
-          softmax_exp16<EMU8, 0>(a, c, nmoff, pka, rs);
-          tmem_ld_wait16(b);
-          if constexpr (MODE & 16) { mbar_wait(b_s2, j & 1); tc_fence_after(); }
-          tmem_ld16(tY, a);
-          softmax_exp16<EMU8, 8>(b, c, nmoff, pka, rs);
-          tmem_ld_wait16(a);
-          tmem_ld16(tY + 16, b);
-          softmax_exp16<EMU8, 0>(a, c, nmoff, pkb, rs);
-          tmem_ld_wait16(b);
-          softmax_exp16<EMU8, 8>(b, c, nmoff, pkb, rs);
-          // Accept the half-tile if its row sum stays below 2^12: then every P <= 2^12 (no fp16 overflow; the relative
-          // precision of P does not depend on its scale), and a sum is what the loop computes anyway -- no maximum over the
-          // scores at all in the common path (33 FMNMX3 less per 64 scores).  inf / NaN sums fail the test too.
-          const float tsum = (rs[0].x + rs[0].y) + (rs[1].x + rs[1].y);
-          redo = __any_sync(0xffffffffu, !(tsum <= 4096.0f)) != 0;
-          if (!redo) {
-            l_run += tsum;
-            tmem_st16(tX, pka);
-            tmem_st16(tX + 16, pkb);
-          }
-        }
-        if (redo) {
-          // the reference moves (always on the first tile).  S is intact in TMEM: pass 1 = row maximum, pass 2 = P.
-          float mxa[4] = {m_ref, m_ref, m_ref, m_ref};
-          if constexpr (MODE & 16) { mbar_wait(b_s2, j & 1); tc_fence_after(); }
-          {
-            tmem_ld16(tX, a);
-            tmem_ld_wait16(a);
-            tmem_ld16(tX + 16, b);
-            rowmax16(a, mxa);
-            tmem_ld_wait16(b);
-            tmem_ld16(tY, a);
-            rowmax16(b, mxa);
-            tmem_ld_wait16(a);
-            tmem_ld16(tY + 16, b);
-            rowmax16(a, mxa);
-            tmem_ld_wait16(b);
-            rowmax16(b, mxa);
-          }
-          const float mx = fmaxf(fmaxf(mxa[0], mxa[1]), fmaxf(mxa[2], mxa[3]));     // >= m_ref
-          const float corr = ex2_approx_ftz((m_ref - mx) * c);                        // m_ref = -inf on the first tile -> 0
-          m_ref = mx;
-          if (j > 0) {
-            mbar_wait(b_o, (j - 1) & 1);            // P_h V_h(j-1) has retired: O_h is complete up to tile j-1
-            tc_fence_after();
-#pragma unroll 1
-            for (int cc = 0; cc < 4; cc++) {
-              tmem_ld16(tO + 16 * cc, a);
-              tmem_ld_wait16(a);
-#pragma unroll
-              for (int i = 0; i < 16; i++) a[i] = __float_as_uint(__uint_as_float(a[i]) * corr);
-              tmem_st16(tO + 16 * cc, a);
-            }
-          }
-          rs[0] = make_float2(0.f, 0.f);
-          rs[1] = make_float2(0.f, 0.f);
-          const float nmoff = -(mx * c);
-          // P is stored (over block X) after every score of the half-tile has been read
-          tmem_ld16(tX, a);
-          tmem_ld_wait16(a);
-          tmem_ld16(tX + 16, b);
-          softmax_exp16<0, 0>(a, c, nmoff, pka, rs);
-          tmem_ld_wait16(b);
-          tmem_ld16(tY, a);
-          softmax_exp16<0, 8>(b, c, nmoff, pka, rs);
-          tmem_ld_wait16(a);
-          tmem_ld16(tY + 16, b);
-          softmax_exp16<0, 0>(a, c, nmoff, pkb, rs);
-          tmem_ld_wait16(b);
-          softmax_exp16<0, 8>(b, c, nmoff, pkb, rs);
-          tmem_st16(tX, pka);
-          tmem_st16(tX + 16, pkb);
-          l_run = l_run * corr + (rs[0].x + rs[0].y) + (rs[1].x + rs[1].y);
-        }
-        if constexpr (MODE & 4) asm volatile("bar.arrive %0, 64;\n" ::"r"(pp_other) : "memory");   // the partner's turn
-        if (q == 0) FA_STAMP(j, 3 * hf + 1);
-        tmem_st_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(b_p);
-        if (q == 0) FA_STAMP(j, 3 * hf + 2);
-      }
-      if constexpr (MODE & 4) {
-        if (hf == 0) asm volatile("bar.sync %0, 64;\n" ::"r"(pp_mine) : "memory");          // consume half 1's last hand-over
-      }
-    } else
-    for (int j = 0; j < nkv; j++) {
-      mbar_wait(b_s, j & 1);
-      tc_fence_after();
-      uint32_t va[32], vb[32];
-      tmem_ld32(tS, va);
-      tmem_ld_wait(va);                            // (wait::ld covers every outstanding load: issue the second one after it)
-      tmem_ld32(tS + 32, vb);
-      float mxa[4] = {m_ref, m_ref, m_ref, m_ref};
-      float2 rs[2] = {make_float2(0.f, 0.f), make_float2(0.f, 0.f)};
-      bool redo = (j == 0);
-      if (!redo) {
-        // optimistic pass against the current reference: exponentials and the tile maximum from one register copy of S
-        const float nmoff = -(m_ref * c);
-#pragma unroll
-        for (int cc = 0; cc < 2; cc++) {
-          uint32_t (&cur)[32] = cc ? vb : va;
-          if (cc) tmem_ld_wait(cur);               // the second half of the scores arrived under the first half's math
-#pragma unroll
-          for (int i = 0; i < 32; i += 2)
-            mxa[(i >> 1) & 3] = fmaxf(mxa[(i >> 1) & 3], fmaxf(__uint_as_float(cur[i]), __uint_as_float(cur[i + 1])));
-          uint32_t pk[16];
-          softmax_exp32<EMU>(cur, c, nmoff, pk, rs);
-          // P_h aliases score columns [0, 32) of this half: those are `va`, already in registers; columns [32, 64) (`vb`,
-          // possibly still being loaded) are never overwritten
-          tmem_st16(tS + 16 * cc, pk);
-        }
-        const float tmax = fmaxf(fmaxf(mxa[0], mxa[1]), fmaxf(mxa[2], mxa[3]));
-        redo = __any_sync(0xffffffffu, (tmax - m_ref) * c > 8.0f) != 0;     // P <= 2^8, else move the reference
-        if (!redo) l_run += (rs[0].x + rs[0].y) + (rs[1].x + rs[1].y);
-      } else {
-        tmem_ld_wait(vb);
-#pragma unroll
-        for (int i = 0; i < 32; i++) mxa[i & 3] = fmaxf(mxa[i & 3], fmaxf(__uint_as_float(va[i]), __uint_as_float(vb[i])));
-      }
-      if (redo) {
-        // the reference moves (always on the first tile): rescale this row's accumulator, redo P from the registers
-        const float mx = fmaxf(fmaxf(mxa[0], mxa[1]), fmaxf(mxa[2], mxa[3]));     // >= m_ref
-        const float corr = ex2_approx_ftz((m_ref - mx) * c);                        // m_ref = -inf on the first tile -> 0
-        m_ref = mx;
-        if (j > 0) {
-          tmem_st_wait();
-          mbar_wait(b_o, (j - 1) & 1);            // P_h V_h(j-1) has retired: O_h is complete up to tile j-1
-          tc_fence_after();
-#pragma unroll 1
-          for (int cc = 0; cc < 4; cc++) {
-            uint32_t v[16];
-            tmem_ld16(tO + 16 * cc, v);
-            tmem_ld_wait16(v);
-#pragma unroll
-            for (int i = 0; i < 16; i++) v[i] = __float_as_uint(__uint_as_float(v[i]) * corr);
-            tmem_st16(tO + 16 * cc, v);
-          }
-        }
-        rs[0] = make_float2(0.f, 0.f);
-        rs[1] = make_float2(0.f, 0.f);
-        const float nmoff = -(mx * c);
-        uint32_t pk[16];
-        softmax_exp32<EMU>(va, c, nmoff, pk, rs);
-        tmem_st16(tS, pk);
-        softmax_exp32<EMU>(vb, c, nmoff, pk, rs);
-        tmem_st16(tS + 16, pk);
-        l_run = l_run * corr + (rs[0].x + rs[0].y) + (rs[1].x + rs[1].y);
-      }
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(b_p);
-    }
-    // ---- merge the two halves of every row through the (idle) K/V ring and write the output ----
-    mbar_wait(b_o, (nkv - 1) & 1);
-    tc_fence_after();
-    // exchange area: the stage NOT used by the last tile (all its MMAs retired before o_full of the last tile fired).
-    // Layout: [half][row 128][32 floats] = 32 KB, 16-byte chunks XOR-swizzled by (row & 7); (m, l) per [half][row] go to the
-    // Q tile (dead as well: every S MMA retired before the last P V did).
-    uint8_t* xbase = smem + (sKV - base) + ((nkv & 1) ? 1 : 0) * 2 * FA_TILE_BYTES;   // stage (nkv-1)%2 is busy -> the other
-    float* xo = reinterpret_cast<float*>(xbase);
-    float2* xml = reinterpret_cast<float2*>(smem);
-    // this thread outputs columns [32 hf, 32 hf + 32) of its row; it hands the other 32 columns of its O_h to the partner
-    {
-      uint32_t v[32];
-      tmem_ld32(tO + 32u * (hf ^ 1), v);
-      tmem_ld_wait(v);
-      float* dstx = xo + ((size_t)hf * 128 + r) * 32;
-#pragma unroll
-      for (int k = 0; k < 8; k++)
-        *reinterpret_cast<uint4*>(dstx + 4 * (k ^ (r & 7))) = make_uint4(v[4 * k], v[4 * k + 1], v[4 * k + 2], v[4 * k + 3]);
-      xml[hf * 128 + r] = make_float2(m_ref, l_run);
-    }
-    asm volatile("bar.sync %0, 64;\n" ::"r"(1 + q) : "memory");
-    const float2 oml = xml[(hf ^ 1) * 128 + r];
-    const float m = fmaxf(m_ref, oml.x);
-    const float e_me = ex2_approx_ftz((m_ref - m) * c), e_ot = ex2_approx_ftz((oml.x - m) * c);
-    const float inv = 1.f / (l_run * e_me + oml.y * e_ot);
-    const float w_me = e_me * inv, w_ot = e_ot * inv;
-    uint32_t v[32];
-    tmem_ld32(tO + 32u * hf, v);
-    tmem_ld_wait(v);
-    const float* srcx = xo + ((size_t)(hf ^ 1) * 128 + r) * 32;
-    __half* dst = p.out + (long long)(row0 + q0 + r) * p.C + h * 64 + 32 * hf;
-#pragma unroll
-    for (int i = 0; i < 32; i += 8) {
-      const float4 o0 = *reinterpret_cast<const float4*>(srcx + 4 * ((i >> 2) ^ (r & 7)));
-      const float4 o1 = *reinterpret_cast<const float4*>(srcx + 4 * (((i >> 2) + 1) ^ (r & 7)));
-      Half8 o8;
-      o8.h[0] = __floats2half2_rn(__uint_as_float(v[i]) * w_me + o0.x * w_ot, __uint_as_float(v[i + 1]) * w_me + o0.y * w_ot);
-      o8.h[1] = __floats2half2_rn(__uint_as_float(v[i + 2]) * w_me + o0.z * w_ot, __uint_as_float(v[i + 3]) * w_me + o0.w * w_ot);
-      o8.h[2] = __floats2half2_rn(__uint_as_float(v[i + 4]) * w_me + o1.x * w_ot, __uint_as_float(v[i + 5]) * w_me + o1.y * w_ot);
-      o8.h[3] = __floats2half2_rn(__uint_as_float(v[i + 6]) * w_me + o1.z * w_ot, __uint_as_float(v[i + 7]) * w_me + o1.w * w_ot);
-      *reinterpret_cast<Half8*>(dst + i) = o8;
-    }
+template <int BN>
+static int launch_fmha(FaParams& fp, const void* qkv, int n_img, int heads, cudaStream_t st) {
+  {
+    cuuint64_t dims[2] = {(cuuint64_t)(3 * fp.C), (cuuint64_t)n_img * (cuuint64_t)fp.L};
+    cuuint64_t str[1] = {(cuuint64_t)(3 * fp.C) * 2};
+    cuuint32_t box[2] = {64, 64};
+    if (encode_map(&fp.q_map, qkv, 2, dims, str, box, nullptr)) return -1;
+    box[1] = BN;
+    if (encode_map(&fp.kv_map, qkv, 2, dims, str, box, nullptr)) return -1;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(tmem_base), "r"(256));
-  }
+  constexpr int smem_max = 2 * FA_QTILE + FA_MAX_STAGES * 2 * BN * 128 + 8 + 16 * FA_MAX_STAGES + 1024;
+  const int smem = 2 * FA_QTILE + fp.stages * 2 * BN * 128 + 8 + 16 * FA_MAX_STAGES + 1024;
+  static bool attr_done[HI3D_MAX_DEVICES];
+  if (ensure_dyn_smem(fmha_tc5_kernel<BN>, smem_max, attr_done, "hi3d_attention_d64_tc5")) return -1;
+  dim3 grid((fp.L + FA_BM - 1) / FA_BM, heads, n_img);
+  fmha_tc5_kernel<BN><<<grid, FA_THREADS, smem, st>>>(fp);
+  return check_launch("hi3d_attention_d64_tc5");
 }
 
 }  // namespace hi3d
 
 using namespace hi3d;
 
-// fraction of the exponentials computed on the FMA pipe: EMU / 4 (0 .. 4; 3 and 4 only in the lean split kernels);
-// -1 = unread (HI3D_FMHA_EMU, else default)
-static int g_fmha_emu = -1;
-constexpr int FA_EMU_DEFAULT = 1;     // measured (profiles/r02_microbench_attn.txt): 1/4 is the optimum of the lean split kernel (837 vs 783 / 794 TFLOP/s for 0 / 2)
-
-extern "C" int hi3d_attention_tc5_set_exp_emulation(int quarters) {
-  if (quarters < 0 || quarters > 7) { set_error("hi3d_attention_tc5_set_exp_emulation: 0 .. 4 (quarters of the exponentials) or 5 / 6 / 7 (3/8, 1/8, 5/8)"); return -2; }
-  g_fmha_emu = quarters;
-  return 0;
-}
-
-// 0 = shared-row kernel, 1 = split half-tile pipelines, 2 = split + register-lean softmax loop, 3 = 2 + the MMA warp serves
-// whichever half is ready, 4 = 2 + ping-pong turns between the halves; -1 = unread (HI3D_FMHA_VARIANT)
-static int g_fmha_variant = -1;
-constexpr int FA_VARIANT_DEFAULT = 2;  // lean split pipelines + 1/4 emulated: 837 vs 774 (split) vs 736 (shared rows) TFLOP/s at L = 16384
-
-extern "C" int hi3d_attention_tc5_set_variant(int variant) {
-  if (variant < 0 || variant > 6) { set_error("hi3d_attention_tc5_set_variant: 0 (shared rows), 1 (split), 2 (split, lean), 3 (split, lean, any-order), 4 (split, lean, ping-pong)"); return -2; }
-  g_fmha_variant = variant;
-  return 0;
-}
-
-static long long* g_fmha_dbg = nullptr;      // device buffer of 128 clock64 stamps for variant 5 (tools only)
-extern "C" int hi3d_attention_tc5_set_debug_buffer(void* buf) { g_fmha_dbg = (long long*)buf; return 0; }
-
-template <int EMU, int MODE>
-static int launch_fmha_split(const FaParams& fp, dim3 grid, cudaStream_t st) {
-  static bool attr_done[HI3D_MAX_DEVICES];
-  if (ensure_dyn_smem(fmha_tc5_split_kernel<EMU, MODE>, FA_SMEM, attr_done, "hi3d_attention_d64_tc5")) return -1;
-  fmha_tc5_split_kernel<EMU, MODE><<<grid, FA_THREADS, FA_SMEM, st>>>(fp);
-  return check_launch("hi3d_attention_d64_tc5");
-}
-
-template <int EMU>
-static int launch_fmha(const FaParams& fp, dim3 grid, cudaStream_t st) {
-  static bool attr_done[HI3D_MAX_DEVICES];
-  if (g_fmha_variant == 5) {
-    if constexpr (EMU == 1) return launch_fmha_split<1, 10>(fp, grid, st);
-    else { set_error("hi3d_attention_d64_tc5: the instrumented variant exists for emulation 1/4 only"); return -2; }
-  }
-  if (g_fmha_variant == 6) return launch_fmha_split<EMU, 18>(fp, grid, st);
-  if (g_fmha_variant == 4) return launch_fmha_split<EMU, 6>(fp, grid, st);
-  if (g_fmha_variant == 3) return launch_fmha_split<EMU, 3>(fp, grid, st);
-  if (g_fmha_variant == 2) return launch_fmha_split<EMU, 2>(fp, grid, st);
-  if constexpr (EMU <= 2) {
-    if (g_fmha_variant == 1) return launch_fmha_split<EMU, 0>(fp, grid, st);
-    if (ensure_dyn_smem(fmha_tc5_kernel<EMU>, FA_SMEM, attr_done, "hi3d_attention_d64_tc5")) return -1;
-    fmha_tc5_kernel<EMU><<<grid, FA_THREADS, FA_SMEM, st>>>(fp);
-    return check_launch("hi3d_attention_d64_tc5");
-  } else {
-    set_error("hi3d_attention_d64_tc5: exp emulation %d/4 needs variant 2 or 3", EMU);
-    return -2;
-  }
-}
-
 extern "C" int hi3d_attention_d64_tc5(const void* qkv, int n_img, int L, int heads, float scale, void* out, void* stream) {
   if (!qkv || !out || n_img <= 0 || L <= 0 || heads <= 0 || ((uintptr_t)qkv & 15) || ((uintptr_t)out & 15)) {
     set_error("hi3d_attention_d64_tc5: bad arguments (n_img=%d L=%d heads=%d)", n_img, L, heads);
     return -2;
   }
-  if ((L % FA_BN) || L < 512 || heads > 65535 || n_img > 65535)   // ragged / short sequences: mma.sync kernel (same results)
-    return hi3d_attention_d64(qkv, n_img, L, heads, scale, out, stream);
+  if (heads > 65535 || n_img > 65535) { set_error("hi3d_attention_d64_tc5: grid too large"); return -2; }
+  read_env_once();
   FaParams fp;
   memset(&fp, 0, sizeof(fp));
-  const int C = heads * 64;
-  {
-    cuuint64_t dims[2] = {(cuuint64_t)(3 * C), (cuuint64_t)n_img * (cuuint64_t)L};
-    cuuint64_t str[1] = {(cuuint64_t)(3 * C) * 2};
-    cuuint32_t box[2] = {64, 128};
-    if (encode_map(&fp.qkv_map, qkv, 2, dims, str, box, nullptr)) return -1;
-  }
-  fp.L = L; fp.C = C; fp.heads = heads;
+  fp.L = L;
+  fp.C = heads * 64;
+  fp.stages = FA_VARIANT_STAGES[g_variant];
+  fp.emu8 = g_emu <= 4 ? 2 * g_emu : (g_emu == 5 ? 3 : (g_emu == 6 ? 1 : 5));
   fp.scale_log2 = scale * 1.4426950408889634f;
   fp.out = (__half*)out;
-  fp.dbg = g_fmha_dbg;
-  if (g_fmha_emu < 0) {
-    const char* e = getenv("HI3D_FMHA_EMU");
-    g_fmha_emu = e ? atoi(e) : FA_EMU_DEFAULT;
-    if (g_fmha_emu < 0 || g_fmha_emu > 7) g_fmha_emu = FA_EMU_DEFAULT;
+  const cudaStream_t st = (cudaStream_t)stream;
+  return FA_VARIANT_BN[g_variant] == 128 ? launch_fmha<128>(fp, qkv, n_img, heads, st) : launch_fmha<64>(fp, qkv, n_img, heads, st);
+}
+
+extern "C" int hi3d_attention_tc5_set_variant(int variant) {
+  if (variant < 0 || variant >= FA_NVARIANTS) {
+    set_error("hi3d_attention_tc5_set_variant: variant must be 0 .. %d", FA_NVARIANTS - 1);
+    return -2;
   }
-  if (g_fmha_variant < 0) {
-    const char* e = getenv("HI3D_FMHA_VARIANT");
-    g_fmha_variant = e ? atoi(e) : FA_VARIANT_DEFAULT;
-    if (g_fmha_variant < 0 || g_fmha_variant > 6) g_fmha_variant = FA_VARIANT_DEFAULT;
+  read_env_once();
+  g_variant = variant;
+  return 0;
+}
+
+extern "C" int hi3d_attention_tc5_set_exp_emulation(int quarters) {
+  if (quarters < 0 || quarters > 7) {
+    set_error("hi3d_attention_tc5_set_exp_emulation: 0 .. 4 (quarters of the exponentials) or 5 / 6 / 7 (3/8, 1/8, 5/8)");
+    return -2;
   }
-  dim3 grid(L / FA_BM, heads, n_img);
-  switch (g_fmha_emu) {
-    case 1: return launch_fmha<1>(fp, grid, (cudaStream_t)stream);
-    case 2: return launch_fmha<2>(fp, grid, (cudaStream_t)stream);
-    case 3: return launch_fmha<3>(fp, grid, (cudaStream_t)stream);
-    case 4: return launch_fmha<4>(fp, grid, (cudaStream_t)stream);
-    case 5: return launch_fmha<5>(fp, grid, (cudaStream_t)stream);
-    case 6: return launch_fmha<6>(fp, grid, (cudaStream_t)stream);
-    case 7: return launch_fmha<7>(fp, grid, (cudaStream_t)stream);
-    default: return launch_fmha<0>(fp, grid, (cudaStream_t)stream);
-  }
+  read_env_once();
+  g_emu = quarters;
+  return 0;
 }

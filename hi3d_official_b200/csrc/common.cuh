@@ -1,4 +1,4 @@
-// Shared device helpers for the Hi3D B200 kernels (sm_100a).
+// Shared device helpers for the Hi3D H100 kernels (sm_90a).
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -63,8 +63,7 @@ HI3D_DEVINL void mma_16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, u
 }
 
 // 128-byte-row shared tile with the 128B XOR swizzle (16-byte chunk index ^= row & 7).  This is the
-// same physical layout tcgen05 SWIZZLE_128B K-major descriptors expect, so the loaders are shared
-// between the mma.sync kernels and the tcgen05 kernels.
+// same physical layout TMA SWIZZLE_128B writes and wgmma SWIZZLE_128B descriptors read.
 HI3D_DEVINL uint32_t swz128(int row, int chunk) { return (uint32_t)(row * 128 + ((chunk ^ (row & 7)) << 4)); }
 
 HI3D_DEVINL uint32_t pack_half2(float a, float b) {

@@ -3,8 +3,7 @@
 // taps, virtual channel-concat, fused nearest-upsample, fused 1x1 skip) -- see include/hi3d_b200.h.
 //
 // Tile: 128 x BN x 64 per CTA, 256 threads (8 warps), STAGES-deep cp.async ring.  Shared tiles use the
-// 128-byte XOR swizzle (common.cuh::swz128) which is also the tcgen05 SWIZZLE_128B K-major layout, so
-// the gather/loader code is shared with the tcgen05 engine (gemm_tc5.cu).
+// 128-byte XOR swizzle (common.cuh::swz128), the same physical layout as a TMA SWIZZLE_128B tile.
 #include <stdarg.h>
 #include <stdio.h>
 
@@ -37,7 +36,7 @@ int device_sm_count() {
   if (cnt[d] <= 0) {
     int v = 0;
     cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, d);
-    cnt[d] = v > 0 ? v : 148;
+    cnt[d] = v > 0 ? v : 132;
   }
   return cnt[d];
 }
@@ -348,6 +347,19 @@ int validate_gemm(const hi3d_gemm_params* p, const char* who) {
   return 0;
 }
 
+// hi3d_gemm_params::gn_stats: a separate statistics pass over the stored tensor.  The four parity-class launches of an
+// up-conv fill one tensor: the pass runs after the last one.
+int gemm_gn_stats_pass(const hi3d_gemm_params* p, void* stream) {
+  if (p->gn_unit <= 0 || (p->N % p->gn_unit) || p->gn_rows <= 0 || (p->M % p->gn_rows) || p->act == HI3D_ACT_GEGLU ||
+      p->out_ld != p->N) {
+    set_error("hi3d_gemm: bad gn_stats arguments (unit %d, rows %d, N %d, out_ld %d)", p->gn_unit, p->gn_rows, p->N, p->out_ld);
+    return -2;
+  }
+  if (p->out_up && !(p->out_py == 1 && p->out_px == 1)) return 0;
+  return hi3d_groupnorm_unit_stats(p->out, p->N, p->M / p->gn_rows, (int64_t)p->gn_rows * (p->out_up ? 4 : 1), p->gn_unit,
+                                   p->gn_stats, stream);
+}
+
 }  // namespace hi3d
 
 using namespace hi3d;
@@ -371,16 +383,7 @@ extern "C" int hi3d_gemm(const hi3d_gemm_params* p, void* stream) {
       rc = wide ? launch_gemm<HI3D_ROWS_TEMPORAL, 128>(*p, st) : launch_gemm<HI3D_ROWS_TEMPORAL, 64>(*p, st);
   }
   if (rc || p->gn_stats == nullptr) return rc;
-  // hi3d_gemm_params::gn_stats on this (first, mma.sync) engine: a separate statistics pass over the stored tensor.  The
-  // four parity-class launches of an up-conv fill one tensor: the pass runs after the last one.
-  if (p->gn_unit <= 0 || (p->N % p->gn_unit) || p->gn_rows <= 0 || (p->M % p->gn_rows) || p->act == HI3D_ACT_GEGLU ||
-      p->out_ld != p->N) {
-    set_error("hi3d_gemm: bad gn_stats arguments (unit %d, rows %d, N %d, out_ld %d)", p->gn_unit, p->gn_rows, p->N, p->out_ld);
-    return -2;
-  }
-  if (p->out_up && !(p->out_py == 1 && p->out_px == 1)) return 0;
-  return hi3d_groupnorm_unit_stats(p->out, p->N, p->M / p->gn_rows, (int64_t)p->gn_rows * (p->out_up ? 4 : 1), p->gn_unit,
-                                   p->gn_stats, stream);
+  return gemm_gn_stats_pass(p, stream);
 }
 
 extern "C" const char* hi3d_last_error(void) { return hi3d::g_err; }

@@ -2,7 +2,7 @@
 // combine in fp64), matching the reference's fp32 GroupNorm32 / autocast-fp32 LayerNorm (SURVEY App. E).
 // Both are pure HBM streams: every thread owns fixed 16-byte channel columns, keeps its per-channel
 // constants in registers and walks rows with several independent 16-byte loads in flight; grids are sized to a
-// few full waves of the 148 SMs.
+// few full waves of the 132 SMs.
 #include "common.cuh"
 
 namespace hi3d {
@@ -10,7 +10,7 @@ namespace hi3d {
 constexpr int GN_MAX_CHUNKS = 512;
 constexpr int GN_GROUPS = 32;
 constexpr int GN_UNROLL = 4;
-constexpr int GN_TARGET_CTAS = 148 * 4 * 4;   // ~4 waves at 4 CTAs/SM
+constexpr int GN_TARGET_CTAS = 132 * 4 * 4;   // ~4 waves at 4 CTAs/SM
 
 HI3D_DEVINL Half8 ld_stream(const __half* p) {
   Half8 v;
@@ -448,7 +448,7 @@ extern "C" int hi3d_groupnorm_apply_halo(const void* x1, int C1, const void* x2,
   const long long max_by_rows = (rows_per_sample + min_rows - 1) / min_rows;
   // 2 CTAs per SM x 3 waves: a CTA lives ~4x longer than with the statistics kernels' grid, so its prologue (group statistics
   // -> mean / rstd -> 16 coefficient registers) is amortised; measured 120 -> see profiles/r02 launch lists
-  long long slabs = (148 * 2 * 3 + n_samples - 1) / n_samples;
+  long long slabs = (132 * 2 * 3 + n_samples - 1) / n_samples;
   if (slabs > max_by_rows) slabs = max_by_rows;
   if (slabs < 1) slabs = 1;
   long long rows_per_cta = (rows_per_sample + slabs - 1) / slabs;

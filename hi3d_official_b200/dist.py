@@ -1,4 +1,4 @@
-"""Multi-GPU plumbing: one process per GPU (`torchrun`), `torch.distributed` (NCCL on B200, gloo in CPU tests).
+"""Multi-GPU plumbing: one process per GPU (`torchrun`), `torch.distributed` (NCCL on H100, gloo in CPU tests).
 
 The hot path shards across GPUs in two ways (SURVEY.md 8e):
   * videos: every rank denoises its own orbital video (BASELINE configs[4]); no data-path collective, only the
@@ -55,7 +55,7 @@ def gather_to_rank0(x: torch.Tensor) -> Optional[torch.Tensor]:
 
 
 # ---- frame-sharded exchanges, NCCL / gloo form -----------------------------------------------------------------------
-# Used by the launch plan (unet._Plan) when HI3D_SHARD_EXCHANGE=nccl; the default on B200 is the peer-memory form
+# Used by the launch plan (unet._Plan) when HI3D_SHARD_EXCHANGE=nccl; the default on H100 is the peer-memory form
 # (peer.py + the sharded kernels), which needs no collective library on the step's path.  These operate in place on the
 # plan's own buffers and are backend-agnostic, so tests/test_dist_cpu.py runs exactly this code under 2-rank gloo.
 def allreduce_sum_(t: torch.Tensor) -> torch.Tensor:

@@ -197,7 +197,7 @@ class VideoLDMStage2(VideoLDM):
 
 
 def create_model(config_path: str, **overrides):
-    """vtdm/model.py:24-28 -- the unmodified reference YAML resolves to the B200 classes through util.TARGET_ALIASES."""
+    """vtdm/model.py:24-28 -- the unmodified reference YAML resolves to the H100 classes through util.TARGET_ALIASES."""
     config = load_yaml(config_path)
     cfg = config["model"]
     params = dict(cfg.get("params", {}))

@@ -111,7 +111,7 @@ class IdentityWrapper(nn.Module):
     def __init__(self, diffusion_model, compile_model: bool = False):
         super().__init__()
         if compile_model:
-            raise NotImplementedError("torch.compile is not part of the B200 path (explicit kernels + CUDA graphs)")
+            raise NotImplementedError("torch.compile is not part of the H100 path (explicit kernels + CUDA graphs)")
         self.diffusion_model = diffusion_model
 
     def forward(self, *args, **kwargs):
@@ -189,7 +189,7 @@ class LinearPredictionGuider:
 # ------------------------------------------------------------------------------------------------------------
 class FusedDenoiser:
     """The pipelines' closure `lambda input, sigma, c: model.denoiser(model.model, input, sigma, c, **kw)`
-    (pipeline_i2v_eval_v01.py:85-88) as an inspectable object, so the sampler can run the fused B200 step.
+    (pipeline_i2v_eval_v01.py:85-88) as an inspectable object, so the sampler can run the fused H100 step.
     Calling it behaves exactly like the closure (generic path)."""
 
     def __init__(self, denoiser: Denoiser, network: nn.Module, shard: Optional[Tuple[int, int]] = None,

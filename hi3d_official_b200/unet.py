@@ -124,7 +124,7 @@ class VideoUNet(nn.Module):
             self.add_module(k, m)
         self._packed: Optional[dict] = None
         self._plans: Dict[tuple, "_Plan"] = {}
-        self.engine = os.environ.get("HI3D_ENGINE", "tc5")     # "tc5" = tcgen05/TMEM/TMA engine, "mma" = mma.sync engine
+        self.engine = os.environ.get("HI3D_ENGINE", "tc5")     # "tc5" = TMA + wgmma engine, "mma" = mma.sync engine
         # packed weights, launch plans and captured graphs derive from the parameters: ANY load that reaches this module
         # -- its own load_state_dict or a parent's (DiffusionEngine.init_from_ckpt recurses through
         # _load_from_state_dict and never calls the override below) -- must drop them
@@ -161,7 +161,7 @@ class VideoUNet(nn.Module):
         sd = {k: v.detach() for k, v in self.state_dict().items()}
         dev = self.device
         if dev.type != "cuda":
-            raise RuntimeError("hi3d_official_b200.VideoUNet computes only on CUDA (B200); call .cuda() first -- "
+            raise RuntimeError("hi3d_official_b200.VideoUNet computes only on CUDA (H100); call .cuda() first -- "
                                "there is no CPU fallback")
         P: dict = {}
         lin, bias = pack.pack_linear, pack.pack_bias

@@ -1,6 +1,6 @@
 """Config / plugin glue: the reference's drop-in seam is `target:` strings resolved by
 `sgm.util.instantiate_from_config` / `get_obj_from_str` (sgm/util.py:168-185).  The same functions here resolve
-the *unmodified* strings of configs/inference-v0{1,2}.yaml to the B200 classes of this package."""
+the *unmodified* strings of configs/inference-v0{1,2}.yaml to the H100 classes of this package."""
 from __future__ import annotations
 
 import importlib

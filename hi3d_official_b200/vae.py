@@ -156,7 +156,7 @@ class _VAEPlan:
         M = n * L
         A = self.A
         if C == 512 and L % 128 == 0 and self.ae.engine == "tc5":
-            # flash attention on tcgen05: q|k|v as ONE GEMM, fp32 scores / softmax inside the kernel, no L x L buffer
+            # flash attention on wgmma: q|k|v as ONE GEMM, fp32 scores / softmax inside the kernel, no L x L buffer
             g, qkv, o = A.want("gn", M, C), A.want("qkv", M, 3 * C), A.want("att", M, C)
             out = self._nxt(M, C)
             self._gn(x, pre + "norm", L, g, silu=False)
@@ -310,7 +310,7 @@ class AutoencoderKL(nn.Module):
             roots[root].put(rest, nn.Parameter(torch.empty(shp), requires_grad=False))
         self._packed = None
         self._plans: Dict[tuple, _VAEPlan] = {}
-        self.engine = os.environ.get("HI3D_ENGINE", "tc5")     # "tc5" = tcgen05/TMEM/TMA engine, "mma" = mma.sync engine
+        self.engine = os.environ.get("HI3D_ENGINE", "tc5")     # "tc5" = TMA + wgmma engine, "mma" = mma.sync engine
         self.max_batch_size = ignored.get("max_batch_size", None)
         # a parent's load_state_dict (DiffusionEngine.init_from_ckpt) recurses through _load_from_state_dict and never
         # reaches the override below: invalidate the packed weights / plans from a pre-hook as well

@@ -1,5 +1,5 @@
 /*
- * hi3d_b200.h -- C ABI of libhi3d_b200.so: the B200 (sm_100a) kernels behind the Hi3D denoising hot path.
+ * hi3d_b200.h -- C ABI of libhi3d_b200.so: the H100 (sm_90a) kernels behind the Hi3D denoising hot path.
  *
  * Boundary (SURVEY.md 8b): the reference is pure Python/PyTorch; its "FFI" for this path is the set of
  * ATen / cuDNN / cuBLAS / xformers calls its nn.Modules make.  Each entry point below replaces one such
@@ -104,18 +104,15 @@ typedef struct {
 } hi3d_gemm_params;
 
 int hi3d_gemm(const hi3d_gemm_params* p, void* stream);
-/* Same contract on the Blackwell-native engine (persistent kernel, TMA operand staging, tcgen05.mma with TMEM
- * accumulators, CTA pairs on long-K shapes): the production path.  Geometries it does not cover (N < 32, unaligned row
- * bias, > 4 distinct A sources, ...) are forwarded to hi3d_gemm, with identical results.
- * Environment (experiments only, read once per process): HI3D_TC5_PAIR=0|1 forces single-CTA / CTA-pair tiles,
- * HI3D_TC5_DBG=<bit mask> disables parts of the kernel for bottleneck measurements (results are then meaningless). */
+/* Same contract on the Hopper-native engine (TMA operand staging through an mbarrier ring, wgmma with register
+ * accumulators, warp-specialised producer / MMA warpgroups): the production path.  Geometries it does not cover (N < 32,
+ * upsample-fused convs, > 4 distinct A sources, ...) are forwarded to hi3d_gemm, with identical results. */
 int hi3d_gemm_tc5(const hi3d_gemm_params* p, void* stream);
-/* Test hook: -1 = automatic choice between single-CTA and CTA-pair (cta_group::2, 256-row) tiles (default, or the value of
- * HI3D_TC5_PAIR at first use), 0 = always single CTA, 1 = always CTA pairs.  Process-wide; the parity tests run every
- * geometry under both settings (no reference counterpart: the reference's cuDNN / cuBLAS pick their own tiles). */
+/* Test / tuning hooks of hi3d_gemm_tc5, process-wide: whether a CTA owns one 128-row tile (8 MMA / epilogue warps) or a pair of
+ * consecutive row tiles sharing each B tile (16 warps, tile widths <= 128).  set_pair_mode: -1 = automatic (default, or
+ * HI3D_TC5_PAIR at first use), 0 = single tiles, 1 = pairs.  set_epilogue_warps: -1 = automatic (default, or HI3D_TC5_EW),
+ * 8 = single tiles, 16 = pairs; a forced pair mode takes precedence. */
 int hi3d_gemm_tc5_set_pair_mode(int mode);
-/* Test / tuning hook: epilogue warps of the specialised bias-only and GEGLU epilogues: -1 = automatic (16 when K <= 640, the
- * GEMMs whose epilogue is the bound), 8 or 16 forced.  Process-wide; default from HI3D_TC5_EW. */
 int hi3d_gemm_tc5_set_epilogue_warps(int warps);
 
 /* Tiny channel counts (UNet input 8|17 ch, VAE image 3 ch / latent 4 ch) are zero-padded to 64 channels by
@@ -186,23 +183,15 @@ int hi3d_layernorm(const void* x, const void* addvec, int add_div, int add_mod, 
  * qkv: fp16 [n_img*L, 3*C] with q | k | v column blocks, heads contiguous (C = heads*64); out fp16 [n_img*L, C].
  * Replaces F.scaled_dot_product_attention / xformers.memory_efficient_attention at attention.py:334,427-439. */
 int hi3d_attention_d64(const void* qkv, int n_img, int L, int heads, float scale, void* out, void* stream);
-/* same contract on tcgen05 / TMEM / TMA (S and P*V accumulators in tensor memory, P fed back from TMEM);
- * sequences that are not a multiple of 128 keys are forwarded to hi3d_attention_d64. */
+/* same contract on TMA + wgmma (S and O accumulators in registers, P fed back to the tensor cores from registers); any L. */
 int hi3d_attention_d64_tc5(const void* qkv, int n_img, int L, int heads, float scale, void* out, void* stream);
-/* Tuning / test hook of hi3d_attention_d64_tc5: `quarters` / 4 of the softmax exponentials (0 .. 4; 3 and 4 only with
- * variants >= 2) are evaluated on the FMA pipe (range reduction + cubic polynomial, relative error 7.5e-5 before the fp16
- * rounding of P) instead of the MUFU pipe.  Process-wide; default from HI3D_FMHA_EMU, else the measured best. */
-int hi3d_attention_tc5_set_exp_emulation(int quarters);
-/* Kernel variant of hi3d_attention_d64_tc5: 0 = eight softmax warps share one score tile, reference maximum and P barrier
- * per CTA; 1 = the 128 keys of a tile are two independent 64-key pipelines (own score / P columns, accumulator, barriers and
- * per-row state), merged once at the end; 2 = 1 with the register-lean softmax loop (scores read in 16-column chunks, P
- * stored once the half-tile is accepted by its row sum); 3 = 2 + the MMA warp serves whichever half is ready; 4 = 2 + strict
- * turns between the halves; 5 = 2 with clock stamps (tools only); 6 = 2 with the scores of a half issued as two 32-key blocks,
- * the first one ahead of P V.  Process-wide; default from HI3D_FMHA_VARIANT, else the
- * measured best. */
+/* Tuning / test hooks of hi3d_attention_d64_tc5, process-wide.  set_variant: 0 .. 6 select the key tile and the depth of the
+ * K/V ring -- (64 keys, 2 stages), (64, 4), (64, 3), (128, 2), (128, 3), (128, 4), (64, 5) = default; default from
+ * HI3D_FMHA_VARIANT.  set_exp_emulation: `quarters` / 4 of the softmax exponentials (0 .. 4; 5 / 6 / 7 = 3/8, 1/8, 5/8) are
+ * evaluated on the FMA pipe (range reduction + cubic, relative error 1.6e-4 before the fp16 rounding of P) instead of MUFU;
+ * default 0, or HI3D_FMHA_EMU. */
 int hi3d_attention_tc5_set_variant(int variant);
-/* tools/fmha_timeline.py: device buffer of 128 int64 that variant 5 fills with clock64 stamps of one CTA; NULL = off. */
-int hi3d_attention_tc5_set_debug_buffer(void* buf);
+int hi3d_attention_tc5_set_exp_emulation(int quarters);
 
 /* Temporal self-attention core over the frame axis (T <= 16), head dim 64, for every (clip, pixel, head):
  * token row of (b, t, s) is (b*T + t)*S + s -- the "(b t) s c -> (b s) t c" rearrange of
@@ -221,7 +210,7 @@ int hi3d_temporal_attention_d64_sharded(void* const* qkv_of_rank, void* const* o
                                         int T_local, int S, int heads, float scale, void* stream);
 
 /* VAE mid-block attention (AttnBlock, model.py:180-201; xformers path model.py:204-265): ONE head of dimension 512,
- * softmax(q k^T * scale) v per image with scale = 512^-0.5, as a flash-attention kernel (tcgen05 / TMEM / TMA): fp32
+ * softmax(q k^T * scale) v per image with scale = 512^-0.5, as a flash-attention kernel (TMA + wgmma): fp32
  * scores and softmax, no L x L matrix in memory.  qkv: fp16 [n_img*L, 1536] = q | k | v column blocks (the three 1x1 convs as
  * one GEMM); out fp16 [n_img*L, 512].  L must be a multiple of 128 ((H/8)*(W/8) at every Hi3D size). */
 int hi3d_attention_d512_tc5(const void* qkv, int n_img, int L, float scale, void* out, void* stream);

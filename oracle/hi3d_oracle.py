@@ -12,7 +12,7 @@ into this oracle (anywhere, CPU or GPU fp32) and into the CUDA product.
 
 Parity pinning: the reference ships NO tests / golden vectors for this path (SURVEY.md F10, §8c), so
 the oracle is pinned against *outputs of the reference itself run in the build container*:
-`tests/test_oracle_vs_reference.py` (runs wherever /root/reference exists) and the committed fixtures
+`tests/test_oracle_vs_reference.py` (against stored outputs of the reference) and the committed fixtures
 `tests/golden/*.pt` produced by `tools/make_golden.py` from the real reference modules.
 
 Numerics: everything is computed in the dtype of the inputs/weights (fp32 on the oracle path); the

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Stage-1 entry point, same CLI as the reference's pipeline_i2v_eval_v01.py (:39-45) on the B200 engine.
+"""Stage-1 entry point, same CLI as the reference's pipeline_i2v_eval_v01.py (:39-45) on the H100 engine.
 
     python pipeline_i2v_eval_v01.py --denoise_config configs/inference-v01.yaml --denoise_checkpoint ckpts/first_stage.pt \
         --image_path demo/15_out.png --output_dir outputs/15_out --elevation 0  [--cond cond.pt | --synthetic]
@@ -129,7 +129,7 @@ def main():
     elif params.synthetic:
         c, uc = synthetic_cond(1, T, h, "cuda", seed)
     else:
-        raise SystemExit("the conditioner towers are outside the B200 hot path: pass --towers / --cond <file> or --synthetic")
+        raise SystemExit("the conditioner towers are outside the H100 hot path: pass --towers / --cond <file> or --synthetic")
     randn = torch.randn(T, 4, h, h, device="cuda")                               # v01:91
     with torch.no_grad():
         frames = model.sample_stage1(c, uc, randn)                               # v01:92-94

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Stage-2 (1024^2 refiner) entry point, same CLI as the reference's pipeline_i2v_eval_v02.py (:38-44) on the B200
+"""Stage-2 (1024^2 refiner) entry point, same CLI as the reference's pipeline_i2v_eval_v02.py (:38-44) on the H100
 engine.  Reads <output_dir>/first_step/first.pt (stage-1 frames written by pipeline_i2v_eval_v01.py; first.mp4 through
 OpenCV when the tensor is absent, like v02:169-176), up-samples them to 1024^2, VAE-encodes each frame (posterior sample,
 CPU RNG like the reference), runs the 25-step re-noise/blend loop of pipeline_i2v_eval_v02.py:127-135 on the fused sampler,
@@ -56,7 +56,7 @@ def main():
     elif params.synthetic:
         c, uc = synthetic_cond(2, T, h, "cuda", seed)
     else:
-        raise SystemExit("the conditioner towers are outside the B200 hot path: pass --towers / --cond <file> or --synthetic")
+        raise SystemExit("the conditioner towers are outside the H100 hot path: pass --towers / --cond <file> or --synthetic")
     with torch.no_grad():
         init_latents = torch.randn(T, 4, h, h, device="cuda")                                      # v02:93
         z = torch.cat([model.encode_first_stage(frames[t:t + 1].half()) for t in range(T)], 0)     # v02:96-101

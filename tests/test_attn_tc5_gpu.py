@@ -1,5 +1,5 @@
-"""tcgen05 / TMEM spatial attention (hi3d_attention_d64_tc5) against PyTorch fp32 softmax(QK^T/8)V and against the
-mma.sync kernel, incl. the ragged-length forwarding path."""
+"""TMA + wgmma spatial attention (hi3d_attention_d64_tc5) against PyTorch fp32 softmax(QK^T/8)V and against the
+mma.sync kernel, incl. sequence lengths that are not a multiple of the key tile."""
 import pytest
 import torch
 
@@ -16,16 +16,16 @@ from test_kernels_gpu import DEV, H, close, rnd  # noqa: E402
                      "blocks-mufu", "blocks-emu25", "blocks-emu37"],
                 autouse=True)
 def kernel_variant(request):
-    """Every case runs on every kernel variant (shared-row CTA / split half-tile pipelines / split with the register-lean
-    softmax loop / the same with any-order MMA service) with part of the softmax exponentials on the FMA pipe (cubic
-    polynomial) -- the production default is one of them (attn_tc5.cu FA_VARIANT_DEFAULT, FA_EMU_DEFAULT)."""
+    """Every case runs on several kernel variants (key tile 64 / 128, K/V ring depth 2 .. 5; the ids keep the names of the
+    project's earlier kernel variants) with part of the softmax exponentials on the FMA pipe (cubic polynomial) -- the
+    production default is one of them (attn_tc5.cu FA_VARIANT_DEFAULT, FA_EMU_DEFAULT)."""
     lib = _native.load()
     variant, emu = request.param
     _native.check(lib.hi3d_attention_tc5_set_variant(variant), "set_variant")
     _native.check(lib.hi3d_attention_tc5_set_exp_emulation(emu), "set_exp_emulation")
     yield request.param
-    _native.check(lib.hi3d_attention_tc5_set_variant(2), "set_variant")            # back to the production defaults
-    _native.check(lib.hi3d_attention_tc5_set_exp_emulation(1), "set_exp_emulation")
+    _native.check(lib.hi3d_attention_tc5_set_variant(6), "set_variant")            # back to the production defaults
+    _native.check(lib.hi3d_attention_tc5_set_exp_emulation(0), "set_exp_emulation")
 
 
 def ref_attn(qkv, n_img, L, heads):
@@ -60,9 +60,8 @@ def test_attention_tc5_ragged_forwards():
 
 @pytest.mark.parametrize("ramp", ["up", "down", "spike"])
 def test_attention_tc5_moving_maximum(ramp):
-    """The softmax reads S once against the running maximum of the previous key tiles and only falls back to
-    max-then-exp when a row grew by more than 2^8: keys whose scores rise, fall or spike along the sequence exercise
-    both paths (and the rescale of the accumulator) inside one call."""
+    """Keys whose scores rise, fall or spike along the sequence: the running maximum of the online softmax moves (and the
+    accumulator is rescaled) many times inside one call."""
     n_img, L, heads = 1, 1024, 2
     C = heads * 64
     qkv = rnd(n_img * L, 3, C)

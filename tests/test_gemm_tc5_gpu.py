@@ -1,4 +1,4 @@
-"""tcgen05/TMEM/TMA implicit-GEMM engine (hi3d_gemm_tc5) against PyTorch fp32 and against the mma.sync engine,
+"""TMA + wgmma implicit-GEMM engine (hi3d_gemm_tc5) against PyTorch fp32 and against the mma.sync engine,
 on every geometry it claims (plain rows, 3x3 conv patches with OOB padding, temporal taps, K-concat, skip
 segments) and every epilogue."""
 import pytest
@@ -15,8 +15,8 @@ E = "tc5"
 
 @pytest.fixture(params=[-1, 8, 16], ids=["ew-auto", "ew8", "ew16"], autouse=True)
 def epilogue_warps(request):
-    """Every case runs with the automatic choice and with 8 / 16 epilogue warps forced (only the specialised bias-only and
-    GEGLU epilogues have a 16-warp build; everything else ignores the setting)."""
+    """Every case runs with the automatic choice and with 8 / 16 MMA + epilogue warps forced (one 128-row tile per CTA, or a
+    pair of row tiles sharing each B tile)."""
     from hi3d_official_b200 import _native
     lib = _native.load()
     _native.check(lib.hi3d_gemm_tc5_set_epilogue_warps(request.param), "set_epilogue_warps")

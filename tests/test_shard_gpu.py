@@ -1,8 +1,7 @@
 """Frame-sharded VideoUNet / fused Euler step over 2 GPUs against the single-GPU result of the same weights, in both
 exchange modes: "peer" (default: pixel-strip temporal attention over peer memory, halo frames stored by the GroupNorm-apply
 kernel into the neighbours' buffers, GroupNorm partial sums on the flag-barrier kernel, whole step under a CUDA graph) and
-"nccl" (K/V all-gather, isend/irecv halo, all-reduce).  Needs >= 2 GPUs (skipped on the 1-GPU box; run with
-`gpurun --gpus 2`, log kept under profiles/)."""
+"nccl" (K/V all-gather, isend/irecv halo, all-reduce).  Needs >= 2 GPUs (skipped on a single GPU)."""
 import os
 
 import pytest
