@@ -13,7 +13,7 @@ from . import build as _build
 
 MAX_SEGS = 24
 ROWS_PLAIN, ROWS_CONV2D, ROWS_TEMPORAL = 0, 1, 2
-ACT_NONE, ACT_SILU, ACT_GEGLU = 0, 1, 2
+ACT_NONE, ACT_SILU, ACT_GEGLU, ACT_GELU, ACT_QUICKGELU = 0, 1, 2, 3, 4
 
 
 class Hi3dError(RuntimeError):
@@ -74,6 +74,7 @@ _SIGS = {
     "hi3d_attention_d64_tc5": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_void_p]),
     "hi3d_attention_tc5_set_exp_emulation": (C.c_int, [C.c_int]),
     "hi3d_attention_tc5_set_variant": (C.c_int, [C.c_int]),
+    "hi3d_attention_d80_tc5": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_void_p]),
     "hi3d_attention_d512_tc5": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_void_p]),
     "hi3d_temporal_attention_d64": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,
                                               C.c_void_p, C.c_void_p]),
@@ -99,6 +100,8 @@ _SIGS = {
                                     C.c_void_p, C.c_void_p]),
     "hi3d_nhwc_to_nchw": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p,
                                     C.c_int, C.c_void_p]),
+    "hi3d_clip_patchify": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
+                                     C.c_void_p]),
     "hi3d_gaussian_sample": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
                                        C.c_float, C.c_void_p, C.c_void_p]),
     "hi3d_pack_weight": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,

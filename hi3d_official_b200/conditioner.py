@@ -8,12 +8,16 @@ that do not need third-party model weights, with the reference's names, ctor kwa
   DepthEmbedder                         vtdm/encoders.py:15-53   (resize, per-image min-max, 3x3 pixel-unshuffle to 9 channels)
   AesEmbedder                           vtdm/encoders.py:56-90   ([score | timestep_embedding(100 score, 255)])
 
-The towers themselves -- OpenCLIP ViT-H (image embedding), MiDaS DPT-hybrid (depth), CLIP ViT-L + aesthetic MLP (score) --
-are third-party networks whose checkpoints are not available offline; they stay OUT of the H100 hot path (SURVEY §2).  Each
-sits behind an `ExternalTower`: a callable installed with `.set_fn(...)`, or a pre-computed tensor passed in the batch under
-`<input_key>:<tower>` (e.g. batch["cond_frames_without_noise:clip"] = (B, 1024)).  Everything AROUND the towers is the
-reference's arithmetic, so the unmodified conditioner_config instantiates and, given tower outputs, produces the reference's
-`c` / `uc` dictionaries (crossattn (B,1,1024), vector (B,768|512), concat (B*T, 4|13, h, w)).
+The image towers -- OpenCLIP ViT-H/14 (image embedding) and OpenAI CLIP ViT-L/14 + the aesthetic MLP (score) -- run natively on
+this package's kernels (clip_vision.py) once their weights are loaded: from the reference's files (the OpenCLIP embedder's
+`version` path; ckpts/ViT-L-14.pt and ckpts/metric_models/sac+logos+ava1-l14-linearMSE.pth relative to the working directory,
+as vtdm/encoders.py:60-64 hard-codes them), or from the `conditioner.embedders.N.*` tensors of a full checkpoint
+(GeneralConditioner.load_tower_weights, called by DiffusionEngine.init_from_ckpt), which win.  MiDaS DPT-hybrid (depth) stays a
+third-party network outside the H100 path.  Every tower sits behind an `ExternalTower`: a callable installed with
+`.set_fn(...)` comes first, then the native tower, and a pre-computed tensor passed in the batch under `<input_key>:<tower>`
+(e.g. batch["cond_frames_without_noise:clip"] = (B, 1024)) takes precedence over both.  Without weights, calling a tower
+raises.  Everything AROUND the towers is the reference's arithmetic, so the unmodified conditioner_config instantiates and
+produces the reference's `c` / `uc` dictionaries (crossattn (B,1,1024), vector (B,768|512), concat (B*T, 4|13, h, w)).
 
 Compatibility: a batch that already holds ready-made dictionaries (`batch["c"]`, optional `batch["uc"]`) is passed through --
 the benches and tests feed synthetic conditioning that way.
@@ -21,6 +25,7 @@ the benches and tests feed synthetic conditioning that way.
 from __future__ import annotations
 
 import math
+import os
 from contextlib import nullcontext
 from typing import Callable, Dict, List, Optional, Sequence, Union
 
@@ -54,7 +59,13 @@ class ExternalTower(AbstractEmbModel):
         self.fn = fn
         return self
 
+    def native(self) -> Optional[Callable]:
+        """The tower on this package's kernels, when its weights are loaded (subclasses)."""
+        return None
+
     def forward(self, x):
+        if self.fn is None and self.native() is not None:
+            return self.native()(x)
         if self.fn is None:
             raise NotImplementedError(
                 f"{type(self).__name__}: this third-party tower (ctor kwargs {self.kwargs}) is outside the H100 hot path and its "
@@ -64,7 +75,33 @@ class ExternalTower(AbstractEmbModel):
 
 
 class FrozenOpenCLIPImageEmbedder(ExternalTower):
-    """sgm/modules/encoders/modules.py:570-728 (OpenCLIP ViT-H-14 image tower -> (N, 1024))."""
+    """sgm/modules/encoders/modules.py:570-728 (OpenCLIP ViT-H-14 image tower -> (N, 1024)): images in [-1, 1] -> kornia bicubic
+    antialiased resize to 224^2 -> [0, 1] -> CLIP normalisation -> ViT.  Native once weights are loaded: at construction from
+    the `version` file when it exists, or later with load_visual()."""
+
+    def __init__(self, *args, **kwargs):
+        super().__init__(*args, **kwargs)
+        self.arch = kwargs.get("arch", "ViT-H-14")
+        self._visual_sd: Optional[Dict[str, torch.Tensor]] = None     # `visual.*` tensors (no prefix), packed on first use
+        self._tower = None
+        version = kwargs.get("version")
+        if isinstance(version, str) and os.path.isfile(version):
+            from . import clip_vision
+            self.load_visual(clip_vision.load_open_clip(version))
+
+    def load_visual(self, sd: Dict[str, torch.Tensor]):
+        self._visual_sd, self._tower = dict(sd), None
+        return self
+
+    def native(self) -> Optional[Callable]:
+        return None if self._visual_sd is None else self._run_native
+
+    def _run_native(self, x: torch.Tensor) -> torch.Tensor:
+        from . import clip_vision
+        if self._tower is None or self._tower.device != x.device:
+            self._tower = clip_vision.ClipVisionTower(self._visual_sd, clip_vision.head_width_of(self.arch), quick_gelu=False,
+                                                      device=x.device)
+        return self._tower(clip_vision.openclip_preprocess(x)).to(x.dtype if x.is_floating_point() else torch.float32)
 
 
 class MiDaSInference(ExternalTower):
@@ -72,7 +109,37 @@ class MiDaSInference(ExternalTower):
 
 
 class AestheticScore(ExternalTower):
-    """vtdm/encoders.py:57-88: CLIP ViT-L image features -> normalised -> aesthetic MLP -> (N, 1) score."""
+    """vtdm/encoders.py:57-88: CLIP ViT-L image features -> normalised -> aesthetic MLP -> (N, 1) score.  Native once weights
+    are loaded: at construction from the reference's files under the working directory when both exist, or later with
+    load_weights()."""
+    CLIP_PATH = os.path.join("ckpts", "ViT-L-14.pt")
+    MLP_PATH = os.path.join("ckpts", "metric_models", "sac+logos+ava1-l14-linearMSE.pth")
+
+    def __init__(self, *args, **kwargs):
+        super().__init__(*args, **kwargs)
+        self._parts = [None, None, None]     # `visual.*` tensors (no prefix), folded MLP weight (768,) and bias ()
+        self._scorer = None
+        if os.path.isfile(self.CLIP_PATH) and os.path.isfile(self.MLP_PATH):
+            from . import clip_vision
+            self.load_weights(clip_vision.load_openai_clip(self.CLIP_PATH), *clip_vision.load_aesthetic_mlp(self.MLP_PATH))
+
+    def load_weights(self, visual_sd: Optional[Dict[str, torch.Tensor]] = None, mlp_w: Optional[torch.Tensor] = None,
+                     mlp_b: Optional[torch.Tensor] = None):
+        """The CLIP tower and the folded MLP may come separately; the scorer is native once both are there."""
+        for i, t in enumerate((visual_sd, mlp_w, mlp_b)):
+            if t is not None:
+                self._parts[i] = dict(t) if isinstance(t, dict) else t
+        self._scorer = None
+        return self
+
+    def native(self) -> Optional[Callable]:
+        return self._run_native if all(t is not None for t in self._parts) else None
+
+    def _run_native(self, x: torch.Tensor) -> torch.Tensor:
+        from . import clip_vision
+        if self._scorer is None or self._scorer.tower.device != x.device:
+            self._scorer = clip_vision.AestheticScorer(*self._parts, device=x.device)
+        return self._scorer(x)
 
 
 def timestep_embedding(t: torch.Tensor, dim: int, max_period: float = 10000.0) -> torch.Tensor:
@@ -243,6 +310,41 @@ class GeneralConditioner(nn.Module):
             embedders.append(embedder)
         self.embedders = nn.ModuleList(embedders)
         self.emb_model_configs = list(emb_models or [])
+
+    # -- native tower weights from a full checkpoint (DiffusionEngine.init_from_ckpt) ---------------------------------------------
+    def load_tower_weights(self, sd: Dict[str, torch.Tensor], prefix: str = "conditioner.") -> List[str]:
+        """Routes `<prefix>embedders.N.open_clip.model.visual.*`, `...N.aesthetic_model.visual.*` and `...N.aesthetic_mlp.*` to the
+        native towers (the reference's module paths).  Returns the names of the towers that received weights."""
+        from . import clip_vision
+        loaded = []
+        for i, e in enumerate(self.embedders):
+            p = f"{prefix}embedders.{i}."
+            if isinstance(e, FrozenOpenCLIPImagePredictionEmbedder) and isinstance(e.open_clip, FrozenOpenCLIPImageEmbedder):
+                vis = {k[len(p + "open_clip.model.visual."):]: v for k, v in sd.items() if k.startswith(p + "open_clip.model.visual.")}
+                if vis:
+                    e.open_clip.load_visual(vis)
+                    loaded.append("clip")
+            elif isinstance(e, AesEmbedder):
+                vis = {k[len(p + "aesthetic_model.visual."):]: v for k, v in sd.items() if k.startswith(p + "aesthetic_model.visual.")}
+                mlp = {k[len(p + "aesthetic_mlp."):]: v for k, v in sd.items() if k.startswith(p + "aesthetic_mlp.")}
+                if vis or mlp:
+                    e.scorer.load_weights(vis or None, *(clip_vision.fold_linear_chain(mlp) if mlp else (None, None)))
+                    loaded.append("aes")
+        return loaded
+
+    def missing_towers(self) -> List[str]:
+        """Towers of this conditioner that can neither run natively nor through an installed callable ('clip', 'depth',
+        'aes'): their outputs must come in the batch."""
+        out = []
+        for e in self.embedders:
+            tower = self.TOWER_OF.get(type(e).__name__)
+            ext = {"clip": lambda m: m.open_clip, "depth": lambda m: m.model, "aes": lambda m: m.scorer}.get(tower)
+            if ext is None:
+                continue
+            t = ext(e)
+            if isinstance(t, ExternalTower) and t.fn is None and t.native() is None:
+                out.append(tower)
+        return out
 
     # -- one embedder, honouring pre-computed tower outputs in the batch -------------------------------------------------------
     def _embed(self, embedder: AbstractEmbModel, batch: Dict):

@@ -75,6 +75,8 @@ HI3D_DEVINL uint32_t pack_half2(float a, float b) {
 // alone was ~10 instructions and made the GroupNorm apply pass issue-bound).  Relative error ~1e-6, output is fp16.
 HI3D_DEVINL float silu_f(float x) { return __fdividef(x, 1.0f + __expf(-x)); }
 HI3D_DEVINL float gelu_erf_f(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752f)); }
+// QuickGELU of OpenAI CLIP (clip/model.py QuickGELU): x * sigmoid(1.702 x), in the form of silu_f.
+HI3D_DEVINL float quick_gelu_f(float x) { return __fdividef(x, 1.0f + __expf(-1.702f * x)); }
 
 HI3D_DEVINL float warp_sum(float v) {
 #pragma unroll
@@ -103,5 +105,23 @@ struct alignas(16) Half8 {
     return *this;
   }
 };
+
+// HI3D_ACT_GELU / HI3D_ACT_QUICKGELU (the CLIP towers' MLP activations) on eight staged fp16 GEMM outputs.  Both GEMM
+// engines apply them in their store pass, on the fp16 tile, before the residual: the register pass that produces the tile
+// (bias, SiLU, GEGLU) is shared by every UNet GEMM, and code added to that unrolled loop slowed those GEMMs down.
+HI3D_DEVINL void clip_act_half8(int act, Half8& v) {
+#pragma unroll
+  for (int q = 0; q < 4; q++) {
+    float2 a = __half22float2(v.h[q]);
+    if (act == HI3D_ACT_GELU) {
+      a.x = gelu_erf_f(a.x);
+      a.y = gelu_erf_f(a.y);
+    } else {
+      a.x = quick_gelu_f(a.x);
+      a.y = quick_gelu_f(a.y);
+    }
+    v.h[q] = __floats2half2_rn(a.x, a.y);
+  }
+}
 
 }  // namespace hi3d

@@ -257,6 +257,7 @@ __global__ void __launch_bounds__(128 + 256 * NT, 1) gemm_tc5_kernel(const __gri
       mo = ((long long)n_ * 2 * p.Ho + 2 * y_ + p.out_py) * (2 * p.Wo) + 2 * x_ + p.out_px;
     }
     Half8 v = *reinterpret_cast<const Half8*>(sC + r * pitch + c * 8);
+    if (p.act >= HI3D_ACT_GELU) clip_act_half8(p.act, v);
     if (p.residual != nullptr) {
       const Half8 rr = *reinterpret_cast<const Half8*>(p.residual + mo * p.res_ld + nc);
 #pragma unroll
@@ -295,13 +296,13 @@ static EncodeTiledFn get_encode() {
 }
 
 int encode_map(CUtensorMap* m, const void* ptr, int rank, const cuuint64_t* dims, const cuuint64_t* strides_bytes,
-               const cuuint32_t* box, const cuuint32_t* elem_strides) {
+               const cuuint32_t* box, const cuuint32_t* elem_strides, CUtensorMapSwizzle swizzle) {
   EncodeTiledFn enc = get_encode();
   if (!enc) { set_error("hi3d_gemm_tc5: cuTensorMapEncodeTiled entry point unavailable"); return -1; }
   cuuint32_t estr[5] = {1, 1, 1, 1, 1};
   if (elem_strides) for (int i = 0; i < rank; i++) estr[i] = elem_strides[i];
   CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, (cuuint32_t)rank, const_cast<void*>(ptr), dims, strides_bytes, box,
-                   estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     set_error("hi3d_gemm_tc5: cuTensorMapEncodeTiled failed (%d) rank=%d dims=%llu,%llu box=%u,%u", (int)r, rank,

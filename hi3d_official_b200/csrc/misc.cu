@@ -255,6 +255,59 @@ extern "C" int hi3d_renoise_blend(float* lat, const float* init, const float* z,
   return check_launch("hi3d_renoise_blend");
 }
 
+// One thread per 8 output columns of one patch row (a 16-byte store); row 0 of each image is the zero class-token slot.
+template <typename TI>
+__global__ void clip_patchify_kernel(const TI* __restrict__ img, int n, int H, int W, int patch, int normalize, int Kpad,
+                                     __half* __restrict__ out) {
+  const int Gx = W / patch, P = (H / patch) * Gx;
+  const int cpr = Kpad / 8, K = 3 * patch * patch, pp = patch * patch;
+  const long long total = (long long)n * (1 + P) * cpr;
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= total) return;
+  const long long row = idx / cpr;
+  const int k0 = (int)(idx - row * cpr) * 8;
+  const int im = (int)(row / (1 + P)), t = (int)(row - (long long)im * (1 + P));
+  const float mean[3] = {0.48145466f, 0.4578275f, 0.40821073f};
+  const float istd[3] = {1.f / 0.26862954f, 1.f / 0.26130258f, 1.f / 0.27577711f};
+  Half8 v;
+#pragma unroll
+  for (int e = 0; e < 8; e += 2) {
+    float a[2];
+#pragma unroll
+    for (int u = 0; u < 2; u++) {
+      const int k = k0 + e + u;
+      float val = 0.f;
+      if (t > 0 && k < K) {
+        const int c = k / pp, r = k - c * pp, ky = r / patch, kx = r - ky * patch;
+        const int py = (t - 1) / Gx, px = (t - 1) - py * Gx;
+        val = (float)img[(((long long)im * 3 + c) * H + py * patch + ky) * W + px * patch + kx];
+        if (normalize) val = (val - mean[c]) * istd[c];
+      }
+      a[u] = val;
+    }
+    v.h[e / 2] = __floats2half2_rn(a[0], a[1]);
+  }
+  *reinterpret_cast<Half8*>(out + row * Kpad + k0) = v;
+}
+
+extern "C" int hi3d_clip_patchify(const void* img, int img_is_fp32, int n, int H, int W, int patch, int normalize, int Kpad,
+                                  void* out, void* stream) {
+  if (!img || !out || n <= 0 || patch <= 0 || H < patch || W < patch || H % patch || W % patch || Kpad % 8 ||
+      Kpad < 3 * patch * patch || ((uintptr_t)out & 15)) {
+    set_error("hi3d_clip_patchify: bad arguments (n=%d H=%d W=%d patch=%d Kpad=%d)", n, H, W, patch, Kpad);
+    return -2;
+  }
+  const long long total = (long long)n * (1 + (H / patch) * (W / patch)) * (Kpad / 8);
+  const int grid = (int)((total + 255) / 256);
+  if (img_is_fp32)
+    clip_patchify_kernel<float><<<grid, 256, 0, (cudaStream_t)stream>>>((const float*)img, n, H, W, patch, normalize, Kpad,
+                                                                      (__half*)out);
+  else
+    clip_patchify_kernel<__half><<<grid, 256, 0, (cudaStream_t)stream>>>((const __half*)img, n, H, W, patch, normalize, Kpad,
+                                                                       (__half*)out);
+  return check_launch("hi3d_clip_patchify");
+}
+
 extern "C" int hi3d_nchw_to_nhwc(const void* in, int in_is_fp32, int N, int C, int H, int W, int Cpad, float scale,
                                  void* out, void* stream) {
   if (!in || !out || N <= 0 || C <= 0 || Cpad < C || (Cpad % 8) || Cpad > 512 || N > 65535) {

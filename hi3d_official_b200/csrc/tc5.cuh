@@ -74,6 +74,17 @@ HI3D_DEVINL uint64_t gmma_desc_sw128(uint32_t smem_addr, uint32_t lbo_bytes = 16
   d |= (uint64_t)1 << 62;
   return d;
 }
+// The same with 32-byte swizzle (layout 3 at bit 62): rows of 16 fp16 (32 B, as TMA SWIZZLE_32B writes a 16-column box), the
+// 16-byte chunk index XORed with bit 2 of the row.  Tiles are 256-byte aligned.  K-major: one row is exactly one 16-wide K
+// step, SBO = 256 B between groups of 8 rows.  MN-major with 16 MN elements: SBO = 256 B between groups of 8 K rows, a
+// 16-row K step is 512 B (+32 in the descriptor).
+HI3D_DEVINL uint64_t gmma_desc_sw32(uint32_t smem_addr) {
+  uint64_t d = (uint64_t)((smem_addr & 0x3FFFF) >> 4);
+  d |= (uint64_t)1 << 16;
+  d |= (uint64_t)(256 >> 4) << 32;
+  d |= (uint64_t)3 << 62;
+  return d;
+}
 HI3D_DEVINL void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
 HI3D_DEVINL void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory"); }
 template <int N>
@@ -147,6 +158,15 @@ HI3D_DEVINL void wgmma_rs_tb<64>(float (&d)[32], const uint32_t (&a)[4], uint64_
 }
 
 template <>
+HI3D_DEVINL void wgmma_rs_tb<16>(float (&d)[8], const uint32_t (&a)[4], uint64_t db, int accumulate) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %13, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1, 1;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate));
+}
+
+template <>
 HI3D_DEVINL void wgmma_rs_tb<256>(float (&d)[128], const uint32_t (&a)[4], uint64_t db, int accumulate) {
   asm volatile(
       "{\n.reg .pred p;\nsetp.ne.b32 p, %133, 0;\n"
@@ -155,8 +175,9 @@ HI3D_DEVINL void wgmma_rs_tb<256>(float (&d)[128], const uint32_t (&a)[4], uint6
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate));
 }
 
-// host: encode a tiled fp16 tensor map with SWIZZLE_128B (defined in gemm_tc5.cu)
+// host: encode a tiled fp16 tensor map, SWIZZLE_128B unless told otherwise (defined in gemm_tc5.cu)
 int encode_map(CUtensorMap* m, const void* ptr, int rank, const cuuint64_t* dims, const cuuint64_t* strides_bytes,
-               const cuuint32_t* box, const cuuint32_t* elem_strides);
+               const cuuint32_t* box, const cuuint32_t* elem_strides,
+               CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B);
 
 }  // namespace hi3d

@@ -4,9 +4,10 @@ vtdm/vtdm_gen_v01.py / vtdm/vtdm_gen_stage2_degradeImage.py, restricted to what 
 reference's key prefixes, `encode_first_stage` / `decode_first_stage`, `.denoiser/.model/.sampler/.conditioner`
 attributes, and the two hot loops (`sample_stage1`, `sample_stage2`) restated on top of the fused sampler.
 
-Out of scope (SURVEY.md section 2): training (`shared_step`, optimisers, EMA, logging) and the third-party conditioner
-towers (OpenCLIP ViT-H, MiDaS, aesthetic MLP).  `PassThroughConditioner` keeps the seam: it returns conditioning
-dictionaries that the caller supplies pre-computed (synthetic in the benches).
+Out of scope (SURVEY.md section 2): training (`shared_step`, optimisers, EMA, logging) and the MiDaS depth tower.  The CLIP
+image towers run natively (clip_vision.py); `init_from_ckpt` hands their `conditioner.embedders.N.*` tensors to the
+conditioner.  `PassThroughConditioner` keeps the seam: it returns conditioning dictionaries that the caller supplies
+pre-computed (synthetic in the benches).
 """
 from __future__ import annotations
 
@@ -80,6 +81,9 @@ class DiffusionEngine(nn.Module):
     def init_from_ckpt(self, path: str) -> None:
         sd = self._read_ckpt(path)
         missing, unexpected = self.load_state_dict(sd, strict=False)
+        towers = self.conditioner.load_tower_weights(sd) if hasattr(self.conditioner, "load_tower_weights") else []
+        if towers:
+            print(f"native conditioner towers from {path}: {towers}")
         unexpected = [k for k in unexpected if not k.startswith(("conditioner.", "loss_fn.", "model_ema."))]
         print(f"Restored from {path} with {len(missing)} missing and {len(unexpected)} unexpected keys")
         if missing:

@@ -12,7 +12,7 @@ from typing import List, Optional, Sequence, Tuple
 import torch
 
 from . import _native as N
-from ._native import ACT_GEGLU, ACT_NONE, ACT_SILU, ROWS_CONV2D, ROWS_PLAIN, ROWS_TEMPORAL  # noqa: F401
+from ._native import ACT_GEGLU, ACT_GELU, ACT_NONE, ACT_QUICKGELU, ACT_SILU, ROWS_CONV2D, ROWS_PLAIN, ROWS_TEMPORAL  # noqa: F401
 
 F16 = torch.float16
 
@@ -217,6 +217,16 @@ def attention_d64(qkv: torch.Tensor, n_img: int, L: int, heads: int, out: torch.
     N.check(fn(qkv.data_ptr(), n_img, L, heads, scale, out.data_ptr(), _stream()), "hi3d_attention_d64")
 
 
+def attention_d80(qkv: torch.Tensor, n_img: int, L: int, heads: int, out: torch.Tensor, scale: float = 80 ** -0.5):
+    """Head dim 80 (OpenCLIP ViT-H/14): qkv fp16 [n_img*L, 3*heads*80] -> out fp16 [n_img*L, heads*80]; any L >= 1."""
+    _chk16(qkv, "qkv"); _chk16(out, "out")
+    C_ = heads * 80
+    if qkv.shape[-1] != 3 * C_ or out.shape[-1] != C_ or qkv.numel() < n_img * L * 3 * C_ or out.numel() < n_img * L * C_:
+        raise ValueError(f"attention_d80: qkv {tuple(qkv.shape)} / out {tuple(out.shape)} do not fit {n_img} x {L} x {heads} heads")
+    N.check(N.load().hi3d_attention_d80_tc5(qkv.data_ptr(), n_img, L, heads, scale, out.data_ptr(), _stream()),
+            "hi3d_attention_d80_tc5")
+
+
 def attention_d512(qkv: torch.Tensor, n_img: int, L: int, out: torch.Tensor, scale: float = 512 ** -0.5):
     """VAE AttnBlock core: one head of dimension 512, qkv fp16 [n_img*L, 1536] -> out fp16 [n_img*L, 512]."""
     _chk16(qkv, "qkv"); _chk16(out, "out")
@@ -316,6 +326,20 @@ def nhwc_to_nchw(x: torch.Tensor, out: torch.Tensor, scale: float = 1.0):
     n, c, h, w = out.shape
     N.check(N.load().hi3d_nhwc_to_nchw(x.data_ptr(), x.shape[-1], n, c, h, w, scale, out.data_ptr(),
                                        int(out.dtype == torch.float32), _stream()), "hi3d_nhwc_to_nchw")
+
+
+def clip_patchify(img: torch.Tensor, patch: int, out: torch.Tensor, normalize: bool = True):
+    """img: contiguous NCHW [n, 3, H, W] fp32 / fp16 -> out fp16 [n * (1 + P), Kpad]: a zero class-token row, then the
+    patches with K ordered (c, ky, kx) (hi3d_clip_patchify)."""
+    if not img.is_cuda or not img.is_contiguous() or img.dtype not in (torch.float32, F16) or img.dim() != 4 or img.shape[1] != 3:
+        raise ValueError("clip_patchify: contiguous CUDA fp32/fp16 NCHW [n, 3, H, W] expected")
+    _chk16(out, "out")
+    n, _, h, w = img.shape
+    rows = n * (1 + (h // patch) * (w // patch))
+    if out.dim() != 2 or out.shape[0] != rows:
+        raise ValueError(f"clip_patchify: out must be [{rows}, Kpad], got {tuple(out.shape)}")
+    N.check(N.load().hi3d_clip_patchify(img.data_ptr(), int(img.dtype == torch.float32), n, h, w, patch, int(normalize),
+                                        out.shape[1], out.data_ptr(), _stream()), "hi3d_clip_patchify")
 
 
 def gaussian_sample(moments: torch.Tensor, noise: Optional[torch.Tensor], out: torch.Tensor, scale: float):

@@ -60,7 +60,9 @@ typedef struct {
 } hi3d_seg;
 
 enum { HI3D_ROWS_PLAIN = 0, HI3D_ROWS_CONV2D = 1, HI3D_ROWS_TEMPORAL = 2 };
-enum { HI3D_ACT_NONE = 0, HI3D_ACT_SILU = 1, HI3D_ACT_GEGLU = 2 };
+/* GELU: exact erf GELU (nn.GELU, open_clip ViT-H MLP); QUICKGELU: x*sigmoid(1.702x) (OpenAI CLIP clip/model.py MLP).  Both are
+ * applied in fp32 to the fp16-rounded value (+ bias) in the epilogue's store pass, before the residual add. */
+enum { HI3D_ACT_NONE = 0, HI3D_ACT_SILU = 1, HI3D_ACT_GEGLU = 2, HI3D_ACT_GELU = 3, HI3D_ACT_QUICKGELU = 4 };
 
 typedef struct {
   int32_t M, N, K;          /* K == sum of seg[i].C; N multiple of 8                                   */
@@ -193,6 +195,12 @@ int hi3d_attention_d64_tc5(const void* qkv, int n_img, int L, int heads, float s
 int hi3d_attention_tc5_set_variant(int variant);
 int hi3d_attention_tc5_set_exp_emulation(int quarters);
 
+/* Same contract for head dim 80 (C = heads*80): the OpenCLIP ViT-H/14 image tower's attention (open_clip transformer.py
+ * nn.MultiheadAttention, 16 heads of 80; the conditioner's FrozenOpenCLIPImageEmbedder, modules.py:570-728).  Any L >= 1;
+ * keys of the next image are masked.  TMA + wgmma, with each 80-column head row staged as a 64-column SWIZZLE_128B box plus a
+ * 16-column SWIZZLE_32B box (no padding of the head dimension). */
+int hi3d_attention_d80_tc5(const void* qkv, int n_img, int L, int heads, float scale, void* out, void* stream);
+
 /* Temporal self-attention core over the frame axis (T <= 16), head dim 64, for every (clip, pixel, head):
  * token row of (b, t, s) is (b*T + t)*S + s -- the "(b t) s c -> (b s) t c" rearrange of
  * video_attention.py:114,137-139 is done by addressing, never materialised.
@@ -262,6 +270,15 @@ int hi3d_nchw_to_nhwc(const void* in, int in_is_fp32, int N, int C, int H, int W
                       void* stream);
 int hi3d_nhwc_to_nchw(const void* in, int in_ld, int N, int C, int H, int W, float scale, void* out, int out_is_fp32,
                       void* stream);
+
+/* Patch rows of a CLIP vision tower (open_clip / OpenAI CLIP VisionTransformer.conv1, a stride = kernel = `patch` conv without
+ * bias, as one plain hi3d_gemm_tc5 against conv1.weight.reshape(width, 3*patch*patch) zero-padded to Kpad columns).
+ * img: NCHW [n, 3, H, W] fp32 or fp16, H and W multiples of `patch`; normalize = 1 applies the CLIP mean / std
+ * ((x - mean) / std, (0.48145466, 0.4578275, 0.40821073) / (0.26862954, 0.26130258, 0.27577711)) on the way.
+ * out: fp16 [n * (1 + P), Kpad], P = (H/patch)*(W/patch): per image an all-zero row (the class-token slot) then the P patches
+ * in raster order, K ordered (c, ky, kx), columns >= 3*patch*patch zero.  Kpad: multiple of 8. */
+int hi3d_clip_patchify(const void* img, int img_is_fp32, int n, int H, int W, int patch, int normalize, int Kpad, void* out,
+                       void* stream);
 
 /* DiagonalGaussianDistribution.sample / mode (distributions.py:24-41,71) * scale_factor (diffusion.py:149):
  * moments fp16 NHWC [N, H, W, ld] (mean = ch 0..C-1, logvar = ch C..2C-1), noise fp32 NCHW or NULL (mode),

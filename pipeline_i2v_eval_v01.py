@@ -4,8 +4,11 @@
     python pipeline_i2v_eval_v01.py --denoise_config configs/inference-v01.yaml --denoise_checkpoint ckpts/first_stage.pt \
         --image_path demo/15_out.png --output_dir outputs/15_out --elevation 0  [--cond cond.pt | --synthetic]
 
-The hot path (25-step fused Euler-EDM over VideoUNet + VAE decode) runs here.  The third-party conditioner towers (rembg,
-OpenCLIP ViT-H, CLIP-L + aesthetic MLP) are outside it; three ways to supply what they produce:
+The hot path (25-step fused Euler-EDM over VideoUNet + VAE decode) runs here.  The conditioner's image towers (OpenCLIP
+ViT-H/14, CLIP ViT-L/14 + aesthetic MLP) run natively when their weights are available -- the reference's files
+(ckpts/open_clip_pytorch_model.bin, ckpts/ViT-L-14.pt, ckpts/metric_models/sac+logos+ava1-l14-linearMSE.pth under the working
+directory) or their tensors inside the checkpoint -- and then --image_path alone builds c / uc through the model's own
+GeneralConditioner, as below.  Otherwise three ways to supply what the towers produce:
   --towers t.pt   {'clip': (1, 1024) image embedding, 'aes': (1, 1) aesthetic score}: the image is pre-processed as in the
                   reference (cv2 resize, centre crop, [-1, 1]; v01:131-149), `add_custom_cond` and the model's own
                   GeneralConditioner (elevation / cond_aug timestep embeddings, VAE-mode latent of the cond frame) build c / uc
@@ -92,14 +95,22 @@ def cond_from_towers(model, frames, towers, elevation, stage):
     batch = {"video": frames[None], "elevation": torch.tensor([float(elevation)], device=frames.device),
              "fps_id": torch.tensor([7.0], device=frames.device), "motion_bucket_id": torch.tensor([127.0], device=frames.device)}
     batch = model.add_custom_cond(batch, infer=True)
-    batch["cond_frames_without_noise:clip"] = towers["clip"].to(frames.device).float().reshape(1, -1)
-    if stage == 1:
+    towers = towers or {}                     # a tower missing here runs natively in the conditioner (or raises)
+    if "clip" in towers:
+        batch["cond_frames_without_noise:clip"] = towers["clip"].to(frames.device).float().reshape(1, -1)
+    if stage == 1 and "aes" in towers:
         batch["video:aes"] = towers["aes"].to(frames.device).float().reshape(1, 1)
-    else:
+    elif stage == 2 and "depth" in towers:
         batch["cond_frames:depth"] = towers["depth"].to(frames.device).float()
     c, uc = model.conditioner.get_unconditional_conditioning(
         batch, force_uc_zero_embeddings=["cond_frames", "cond_frames_without_noise"])
     return c, uc
+
+
+def native_towers_ready(model, allowed_missing=()):
+    """True when the model's GeneralConditioner runs every tower natively (weights loaded), except `allowed_missing`."""
+    missing = getattr(model.conditioner, "missing_towers", None)
+    return missing is not None and not set(missing()) - set(allowed_missing)
 
 
 def main():
@@ -128,6 +139,9 @@ def main():
         c, uc = cond_from_towers(model, img[:, None].repeat(1, T, 1, 1), torch.load(params.towers), params.elevation, 1)
     elif params.synthetic:
         c, uc = synthetic_cond(1, T, h, "cuda", seed)
+    elif native_towers_ready(model):
+        img = load_image(params.image_path, 8 * h).cuda()
+        c, uc = cond_from_towers(model, img[:, None].repeat(1, T, 1, 1), None, params.elevation, 1)
     else:
         raise SystemExit("the conditioner towers are outside the H100 hot path: pass --towers / --cond <file> or --synthetic")
     randn = torch.randn(T, 4, h, h, device="cuda")                               # v01:91

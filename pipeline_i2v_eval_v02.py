@@ -4,7 +4,8 @@ engine.  Reads <output_dir>/first_step/first.pt (stage-1 frames written by pipel
 OpenCV when the tensor is absent, like v02:169-176), up-samples them to 1024^2, VAE-encodes each frame (posterior sample,
 CPU RNG like the reference), runs the 25-step re-noise/blend loop of pipeline_i2v_eval_v02.py:127-135 on the fused sampler,
 decodes and writes second_step_video/second.mp4.  Conditioning: --towers {'clip': (1,1024), 'depth': (T,h',w') MiDaS maps} /
---cond / --synthetic as in v01; --tiny = the smoke size the tests run."""
+--cond / --synthetic as in v01; 'clip' may be left out of --towers when the OpenCLIP tower's weights are available (it then
+runs natively in the conditioner; MiDaS depth always comes from --towers); --tiny = the smoke size the tests run."""
 import argparse
 import os
 import random
