@@ -1,15 +1,26 @@
-// Spatial self-attention core (head dim 64) on Hopper: TMA operand staging through an mbarrier ring and wgmma for both
-// products -- S = Q K^T with Q and K from shared memory, O += P V with P from registers (the S accumulator fragment is the
-// A-operand fragment of the next product, so P never touches shared memory) and V as an MN-major shared-memory operand.
+// Spatial self-attention core (head dim 64) on Hopper: a warp-specialised, software-pipelined flash-attention kernel.
+// TMA stages the operands through mbarrier rings and wgmma runs both products -- S = Q K^T with Q and K from shared memory,
+// O += P V with P from registers (the S accumulator fragment is the A-operand fragment of the next product, so P never
+// touches shared memory) and V as an MN-major shared-memory operand.
 //
-// CTA = 128 queries x one (image, head), two warpgroups of 64 query rows; keys stream in tiles of BN (64 or 128) through a
-// ring of (K, V) tiles that both warpgroups read.  Thread 0 issues every TMA load; each warp releases a stage once its
-// warpgroup's MMAs on it have retired.  The key tail (L not a multiple of BN: keys of the next image or TMA out-of-bounds
-// zeros) is masked to -inf before the online softmax; query rows past L are computed and not stored.
+// CTA = 64 NC queries x one (image, head): warpgroup 0 is the producer (one lane issues every TMA load and the warpgroup
+// hands its registers to the consumers), warpgroups 1 .. NC each own 64 query rows.  Keys stream in tiles of BN (64 or
+// 128) through two rings, one of K tiles and one of V tiles, each stage with its own full and empty barrier: S_j starts as
+// soon as K_j has landed, K_j's slot goes back to the producer when S_j retires and V_j's when P_j V_j retires.
 //
-// Variants (hi3d_attention_tc5_set_variant) choose the key tile and the ring depth; hi3d_attention_tc5_set_exp_emulation
-// moves a fraction (quarters, or 1/8, 3/8, 5/8) of the softmax exponentials from the MUFU pipe to the FMA pipe (exp2 by range reduction and a
-// cubic, relative error 1.6e-4 before the fp16 rounding of P).
+// At d = 64 the exponentials (MUFU) take as many cycles as the two products (tensor cores), so a consumer overlaps them:
+//   issue S_j = Q K_j^T | O *= correction_{j-1} | issue O += P_{j-1} V_{j-1} | wait S_j | softmax(S_j) | wait P V | pack P_j
+// -- the softmax of tile j runs while the tensor cores work on S_j's tail and on P_{j-1} V_{j-1}.  Only wgmma touches the
+// registers of an in-flight product (P_j stays fp32 in the S registers until P_{j-1} V_{j-1} retires), so ptxas keeps the
+// products asynchronous.
+//
+// The key tail (L not a multiple of BN: keys of the next image or TMA out-of-bounds zeros) is masked to -inf before the
+// online softmax; tiles are visited in order, so the masked tile comes last and every row has a finite maximum by then.
+// Query rows past L are computed and not stored.
+//
+// Variants (hi3d_attention_tc5_set_variant) choose the key tile, the consumer count and the ring depth;
+// hi3d_attention_tc5_set_exp_emulation moves a fraction (quarters, or 1/8, 3/8, 5/8) of the softmax exponentials from the
+// MUFU pipe to the FMA pipe (exp2 by range reduction and a cubic, relative error 1.6e-4 before the fp16 rounding of P).
 #include <cuda.h>
 #include <stdlib.h>
 #include <string.h>
@@ -19,25 +30,28 @@
 
 namespace hi3d {
 
-constexpr int FA_BM = 128;                 // queries per CTA
-constexpr int FA_MAX_STAGES = 5;
-constexpr int FA_THREADS = 256;
-constexpr int FA_QTILE = 64 * 128;         // 64 rows x 64 fp16
+constexpr int FA_MAX_STAGES = 4;
+constexpr int FA_QTILE = 64 * 128;         // 64 query rows x 64 fp16: one consumer warpgroup's Q tile
 
 struct FaParams {
   CUtensorMap q_map;       // [n_img * L, 3C] fp16 (q | k | v), box {64, 64}
   CUtensorMap kv_map;      // the same matrix, box {64, BN}
-  int L, C, stages, emu8;   // emu8: eighths of the exponentials on the FMA pipe
+  int L, C, stages;
   float scale_log2;
   __half* out;             // [n_img * L, C]
 };
 
-// (key tile, ring depth) of each variant.  Default: variant 6 without exponential emulation, the fastest on an H100 at the
-// benchmark's shapes (32 images x 5 heads, L = 16384: 290 TFLOP/s against 272 for (64, 3) and 225 for the 128-key tiles;
-// L = 4096: 288 against 280).
+// (key tile, consumer warpgroups, ring depth) of each variant.  Default: variant 6 without exponential emulation.  On an
+// H100 80GB HBM3 at 700 W (tools/time_attention.py, 32 images): L = 16384 x 5 heads 413 TFLOP/s (variant 5: 417, 4: 412,
+// 2: 408, 3: 407, the two-stage 64-key variants 0 / 1: 350), L = 4096 x 10 heads 391 (5: 393), L = 1024 x 20 heads 334
+// (5: 318), L = 256 x 20 heads 194 (5: 164) -- variant 6 is within 1 % of the fastest at every shape.  Moving 1/8 of the
+// exponentials to the FMA pipe costs 8 % at L = 16384 and 3/8 costs 14 %: the tensor cores, not MUFU, set the pace now.
 constexpr int FA_NVARIANTS = 7;
-constexpr int FA_VARIANT_BN[FA_NVARIANTS] = {64, 64, 64, 128, 128, 128, 64};
-constexpr int FA_VARIANT_STAGES[FA_NVARIANTS] = {2, 4, 3, 2, 3, 4, 5};
+// 128-key tiles run with two consumers only: three need S (64) + P (32) + O (32) fp32 registers per thread in flight, and
+// ptxas allocates to the 128-register cap of a 512-thread CTA (not to the setmaxnreg budget), so they spill.
+constexpr int FA_VARIANT_BN[FA_NVARIANTS] = {64, 64, 64, 128, 128, 64, 128};
+constexpr int FA_VARIANT_NC[FA_NVARIANTS] = {2, 2, 3, 2, 2, 3, 2};
+constexpr int FA_VARIANT_STAGES[FA_NVARIANTS] = {2, 4, 2, 2, 4, 4, 3};
 constexpr int FA_VARIANT_DEFAULT = 6;
 constexpr int FA_EMU_DEFAULT = 0;
 
@@ -50,127 +64,203 @@ HI3D_DEVINL float exp2_fma(float x) {
   return __int_as_float(__float_as_int(p) + ((int)j << 23));
 }
 
+// 2^x on the MUFU pipe.  exp2f adds a range test and two multiplies around MUFU.EX2 to produce denormal results; P is
+// rounded to fp16 (which flushes them to zero anyway) and the row sums are >= 1, so the flush-to-zero form loses nothing.
+HI3D_DEVINL float exp2_mufu(float x) {
+  float y;
+  asm("ex2.approx.ftz.f32 %0, %1;\n" : "=f"(y) : "f"(x));
+  return y;
+}
+
+// Online softmax of one S tile (key tile j) in place: masks the key tail, updates the running max / sum of this thread's
+// rows g (hh = 0) and g + 8 (hh = 1) of its warp's 16, leaves P (fp32) in the S registers and returns the factor by which
+// the accumulator must be rescaled.  P is packed into the A fragments of P V separately (fa_pack), once the previous P V
+// that reads those registers has retired.
+// EMU8: eighths of the key columns whose exponentials run on the FMA pipe -- a template parameter, so that each column's
+// pipe is fixed at compile time (a run-time fraction made every exponential compute both forms and select one).
+template <int BN, int EMU8>
+HI3D_DEVINL void fa_softmax(float (&sc)[BN / 2], float (&mrow)[2], float (&lrow)[2], float (&corr)[2], int j, int L,
+                            float c, int t4) {
+  if ((j + 1) * BN > L) {
+#pragma unroll
+    for (int nt = 0; nt < BN / 8; nt++) {
+      const int col = j * BN + nt * 8 + 2 * t4;
+      if (col >= L) { sc[4 * nt] = -INFINITY; sc[4 * nt + 2] = -INFINITY; }
+      if (col + 1 >= L) { sc[4 * nt + 1] = -INFINITY; sc[4 * nt + 3] = -INFINITY; }
+    }
+  }
+#pragma unroll
+  for (int hh = 0; hh < 2; hh++) {
+    float mx = -INFINITY;
+#pragma unroll
+    for (int nt = 0; nt < BN / 8; nt++) mx = fmaxf(mx, fmaxf(sc[4 * nt + 2 * hh], sc[4 * nt + 2 * hh + 1]));
+    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+    const float mnew = fmaxf(mrow[hh], mx);
+    corr[hh] = exp2_mufu((mrow[hh] - mnew) * c);
+    const float moff = mnew * c;
+    float rs = 0.f;
+#pragma unroll
+    for (int nt = 0; nt < BN / 8; nt++) {
+      const float x0 = sc[4 * nt + 2 * hh] * c - moff, x1 = sc[4 * nt + 2 * hh + 1] * c - moff;
+      const bool fma_pipe = (nt & 7) < EMU8;
+      const float p0 = fma_pipe ? exp2_fma(x0) : exp2_mufu(x0);
+      const float p1 = fma_pipe ? exp2_fma(x1) : exp2_mufu(x1);
+      rs += p0 + p1;
+      sc[4 * nt + 2 * hh] = p0;
+      sc[4 * nt + 2 * hh + 1] = p1;
+    }
+    lrow[hh] = lrow[hh] * corr[hh] + rs;
+    mrow[hh] = mnew;
+  }
+}
+
+// accumulator fragment -> A fragment: key columns 8 nt .. feed k16 step nt / 2, registers (nt & 1) * 2 + hh
 template <int BN>
-__global__ void __launch_bounds__(FA_THREADS, 1) fmha_tc5_kernel(const __grid_constant__ FaParams p) {
+HI3D_DEVINL void fa_pack(const float (&sc)[BN / 2], uint32_t (&pa)[BN / 16][4]) {
+#pragma unroll
+  for (int nt = 0; nt < BN / 8; nt++)
+#pragma unroll
+    for (int hh = 0; hh < 2; hh++) pa[nt >> 1][(nt & 1) * 2 + hh] = pack_half2(sc[4 * nt + 2 * hh], sc[4 * nt + 2 * hh + 1]);
+}
+
+template <int BN, int NC, int EMU8>
+__global__ void __launch_bounds__(128 * (NC + 1), 1) fmha_tc5_kernel(const __grid_constant__ FaParams p) {
   constexpr int KV_TILE = BN * 128;
+  constexpr int BM = 64 * NC;                                // queries per CTA
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
   uint8_t* smem = smem_raw + (base - raw);
   const int STAGES = p.stages;
-  const uint32_t sQ = base;                                  // [128 queries x 64]
-  const uint32_t sR = base + 2 * FA_QTILE;                   // ring: STAGES x (K tile, V tile)
-  const uint32_t bar_q = sR + STAGES * 2 * KV_TILE;
-  const uint32_t bar_full = bar_q + 8;                       // [STAGES]
-  const uint32_t bar_empty = bar_full + 8 * FA_MAX_STAGES;   // [STAGES], one arrive per warp
+  const uint32_t sQ = base;                                  // NC x [64 queries x 64]
+  const uint32_t sK = sQ + NC * FA_QTILE;                    // STAGES K tiles
+  const uint32_t sV = sK + STAGES * KV_TILE;                 // STAGES V tiles
+  const uint32_t bar_q = sV + STAGES * KV_TILE;
+  const uint32_t bar_kfull = bar_q + 8;                      // [STAGES] each: the producer's expect_tx arrive
+  const uint32_t bar_vfull = bar_kfull + 8 * FA_MAX_STAGES;
+  const uint32_t bar_kempty = bar_vfull + 8 * FA_MAX_STAGES; // [STAGES] each: one arrive per consumer warp
+  const uint32_t bar_vempty = bar_kempty + 8 * FA_MAX_STAGES;
 
   const int tid = threadIdx.x, lane = tid & 31;
-  const int cw = tid >> 7;                                   // warpgroup: query rows 64 cw .. + 63
-  const int warp = (tid >> 5) & 3;
-  const int q0 = blockIdx.x * FA_BM;
+  const int wg = __shfl_sync(0xffffffffu, tid >> 7, 0);      // warp-uniform role index
+  const int q0 = blockIdx.x * BM;
   const int h = blockIdx.y;
   const int row0 = blockIdx.z * p.L;
   const int nkv = (p.L + BN - 1) / BN;
   const int C = p.C;
 
-  auto issue_kv = [&](int j, int s) {
-    const uint32_t full = bar_full + 8 * s;
-    mbar_expect_tx(full, 2 * KV_TILE);
-    tma_load_2d(sR + s * 2 * KV_TILE, &p.kv_map, full, C + h * 64, row0 + j * BN);
-    tma_load_2d(sR + s * 2 * KV_TILE + KV_TILE, &p.kv_map, full, 2 * C + h * 64, row0 + j * BN);
-  };
   if (tid == 0) {
     mbar_init(bar_q, 1);
-    for (int s = 0; s < STAGES; s++) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, 8); }
+    for (int s = 0; s < STAGES; s++) {
+      mbar_init(bar_kfull + 8 * s, 1);
+      mbar_init(bar_vfull + 8 * s, 1);
+      mbar_init(bar_kempty + 8 * s, 4 * NC);
+      mbar_init(bar_vempty + 8 * s, 4 * NC);
+    }
     asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
-    mbar_expect_tx(bar_q, 2 * FA_QTILE);
-    tma_load_2d(sQ, &p.q_map, bar_q, h * 64, row0 + q0);
-    tma_load_2d(sQ + FA_QTILE, &p.q_map, bar_q, h * 64, row0 + q0 + 64);
-    for (int j = 0; j < STAGES && j < nkv; j++) issue_kv(j, j);
   }
   __syncthreads();
 
+  if (wg == 0) {
+    // ======================= TMA producer: Q once, then K_0, and (K_{j+1}, V_j) in the order the consumers use them
+    setmaxnreg_dec<NC == 2 ? 24 : 32>();
+    if (tid == 0) {
+      mbar_expect_tx(bar_q, NC * FA_QTILE);
+      for (int c = 0; c < NC; c++) tma_load_2d(sQ + c * FA_QTILE, &p.q_map, bar_q, h * 64, row0 + q0 + 64 * c);
+      uint32_t ks = 0, kph = 0, vs = 0, vph = 0;
+      auto load_k = [&](int j) {
+        mbar_wait(bar_kempty + 8 * ks, kph ^ 1);
+        mbar_expect_tx(bar_kfull + 8 * ks, KV_TILE);
+        tma_load_2d(sK + ks * KV_TILE, &p.kv_map, bar_kfull + 8 * ks, C + h * 64, row0 + j * BN);
+        if (++ks == (uint32_t)STAGES) { ks = 0; kph ^= 1; }
+      };
+      load_k(0);
+      for (int j = 0; j < nkv; j++) {
+        if (j + 1 < nkv) load_k(j + 1);
+        mbar_wait(bar_vempty + 8 * vs, vph ^ 1);
+        mbar_expect_tx(bar_vfull + 8 * vs, KV_TILE);
+        tma_load_2d(sV + vs * KV_TILE, &p.kv_map, bar_vfull + 8 * vs, 2 * C + h * 64, row0 + j * BN);
+        if (++vs == (uint32_t)STAGES) { vs = 0; vph ^= 1; }
+      }
+    }
+    return;
+  }
+
+  // ======================= consumers: warpgroup cw owns query rows 64 cw .. + 63 of the CTA's tile
+  setmaxnreg_inc<NC == 2 ? 240 : 160>();
+  const int cw = wg - 1;
+  const int warp = (tid >> 5) & 3;
   float o[32];
 #pragma unroll
   for (int i = 0; i < 32; i++) o[i] = 0.f;
-  float mrow[2] = {-INFINITY, -INFINITY}, lrow[2] = {0.f, 0.f};
+  float mrow[2] = {-INFINITY, -INFINITY}, lrow[2] = {0.f, 0.f}, corr[2];
   const int t4 = lane & 3;
   const float c = p.scale_log2;
   const uint64_t qd = gmma_desc_sw128(sQ + cw * FA_QTILE);
-  const int emu8 = p.emu8;
-  mbar_wait(bar_q, 0);
-
-  uint32_t s = 0, ph = 0;
-  for (int j = 0; j < nkv; j++) {
-    mbar_wait(bar_full + 8 * s, ph);
-    const uint32_t sK = sR + s * 2 * KV_TILE, sV = sK + KV_TILE;
-    // ---- S = Q K^T ----
-    float sc[BN / 2];
-    const uint64_t kd = gmma_desc_sw128(sK);
+  float sc[BN / 2];
+  uint32_t pa[BN / 16][4];
+  uint32_t ks = 0, kph = 0, vs = 0, vph = 0;
+  auto issue_s = [&]() {       // S = Q K^T on K stage ks
+    const uint64_t kd = gmma_desc_sw128(sK + ks * KV_TILE);
     wgmma_fence();
 #pragma unroll
     for (int k = 0; k < 4; k++) wgmma_ss<BN>(sc, qd + (uint64_t)(2 * k), kd + (uint64_t)(2 * k), k);
     wgmma_commit();
-    wgmma_wait<0>();
-    wgmma_fence_regs(sc);
-    // ---- mask the key tail ----
-    if ((j + 1) * BN > p.L) {
-#pragma unroll
-      for (int nt = 0; nt < BN / 8; nt++) {
-        const int col = j * BN + nt * 8 + 2 * t4;
-        if (col >= p.L) { sc[4 * nt] = -INFINITY; sc[4 * nt + 2] = -INFINITY; }
-        if (col + 1 >= p.L) { sc[4 * nt + 1] = -INFINITY; sc[4 * nt + 3] = -INFINITY; }
-      }
-    }
-    // ---- online softmax: this thread holds rows g (hh = 0) and g + 8 (hh = 1) of its warp's 16 rows ----
-    uint32_t pa[BN / 16][4];
-#pragma unroll
-    for (int hh = 0; hh < 2; hh++) {
-      float mx = -INFINITY;
-#pragma unroll
-      for (int nt = 0; nt < BN / 8; nt++) mx = fmaxf(mx, fmaxf(sc[4 * nt + 2 * hh], sc[4 * nt + 2 * hh + 1]));
-      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
-      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
-      const float mnew = fmaxf(mrow[hh], mx);
-      const float corr = exp2f((mrow[hh] - mnew) * c);
-      const float moff = mnew * c;
-      float rs = 0.f;
-#pragma unroll
-      for (int nt = 0; nt < BN / 8; nt++) {
-        const float x0 = sc[4 * nt + 2 * hh] * c - moff, x1 = sc[4 * nt + 2 * hh + 1] * c - moff;
-        const bool fma_pipe = (nt & 7) < emu8;       // emu8 eighths of the key columns
-        const float p0 = fma_pipe ? exp2_fma(x0) : exp2f(x0);
-        const float p1 = fma_pipe ? exp2_fma(x1) : exp2f(x1);
-        rs += p0 + p1;
-        // accumulator fragment -> A fragment: key columns 8 nt .. feed k16 step nt / 2, register (nt & 1) * 2 + hh
-        pa[nt >> 1][(nt & 1) * 2 + hh] = pack_half2(p0, p1);
-      }
-      lrow[hh] = lrow[hh] * corr + rs;
-      mrow[hh] = mnew;
-#pragma unroll
-      for (int dt = 0; dt < 8; dt++) {
-        o[4 * dt + 2 * hh] *= corr;
-        o[4 * dt + 2 * hh + 1] *= corr;
-      }
-    }
-    // ---- O += P V (16 keys per MMA: V advances 16 rows = 2048 bytes) ----
-    const uint64_t vd = gmma_desc_sw128(sV);
+  };
+  auto issue_pv = [&]() {      // O += P V on V stage vs (16 keys per MMA: V advances 16 rows = 2048 bytes)
+    const uint64_t vd = gmma_desc_sw128(sV + vs * KV_TILE);
     wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < BN / 16; kk++) wgmma_rs_tb<64>(o, pa[kk], vd + (uint64_t)(128 * kk), 1);
     wgmma_commit();
+  };
+  auto release = [&](uint32_t bar, uint32_t& s, uint32_t& ph) {
+    __syncwarp();
+    if (lane == 0) mbar_arrive(bar + 8 * s);
+    if (++s == (uint32_t)STAGES) { s = 0; ph ^= 1; }
+  };
+
+  auto rescale_o = [&]() {
+#pragma unroll
+    for (int dt = 0; dt < 8; dt++) {
+      o[4 * dt] *= corr[0];
+      o[4 * dt + 1] *= corr[0];
+      o[4 * dt + 2] *= corr[1];
+      o[4 * dt + 3] *= corr[1];
+    }
+  };
+
+  mbar_wait(bar_q, 0);
+  mbar_wait(bar_kfull, 0);
+  issue_s();
+  wgmma_wait<0>();
+  wgmma_fence_regs(sc);
+  release(bar_kempty, ks, kph);
+  fa_softmax<BN, EMU8>(sc, mrow, lrow, corr, 0, p.L, c, t4);
+  fa_pack<BN>(sc, pa);
+  for (int j = 1; j < nkv; j++) {
+    mbar_wait(bar_kfull + 8 * ks, kph);
+    issue_s();                                  // S_j
+    rescale_o();                                // to tile j - 1's running max
+    mbar_wait(bar_vfull + 8 * vs, vph);
+    issue_pv();                                 // O += P_{j-1} V_{j-1}
+    wgmma_wait<1>();                            // S_j has retired, P V may still run
+    wgmma_fence_regs(sc);
+    release(bar_kempty, ks, kph);
+    fa_softmax<BN, EMU8>(sc, mrow, lrow, corr, j, p.L, c, t4);
     wgmma_wait<0>();
     wgmma_fence_regs(o);
-    __syncwarp();
-    if (lane == 0) mbar_arrive(bar_empty + 8 * s);
-    if (tid == 0 && j + STAGES < nkv) {
-      mbar_wait(bar_empty + 8 * s, ph);          // both warpgroups are done with this stage
-      issue_kv(j + STAGES, s);
-    }
-    if (++s == (uint32_t)STAGES) { s = 0; ph ^= 1; }
+    release(bar_vempty, vs, vph);
+    fa_pack<BN>(sc, pa);
   }
+  rescale_o();
+  mbar_wait(bar_vfull + 8 * vs, vph);
+  issue_pv();
+  wgmma_wait<0>();
+  wgmma_fence_regs(o);
 
-  // ---- finalize: O /= l, stage through this warpgroup's own Q rows, 16-byte stores ----
+  // ---- finalize: O /= l, stage through this warpgroup's own Q rows (only its own S products read them), 16-byte stores
   const int g = lane >> 2;
   uint8_t* stage = smem + cw * FA_QTILE;
 #pragma unroll
@@ -213,7 +303,7 @@ static void read_env_once() {
   }
 }
 
-template <int BN>
+template <int BN, int NC, int EMU8>
 static int launch_fmha(FaParams& fp, const void* qkv, int n_img, int heads, cudaStream_t st) {
   {
     cuuint64_t dims[2] = {(cuuint64_t)(3 * fp.C), (cuuint64_t)n_img * (cuuint64_t)fp.L};
@@ -223,13 +313,21 @@ static int launch_fmha(FaParams& fp, const void* qkv, int n_img, int heads, cuda
     box[1] = BN;
     if (encode_map(&fp.kv_map, qkv, 2, dims, str, box, nullptr)) return -1;
   }
-  constexpr int smem_max = 2 * FA_QTILE + FA_MAX_STAGES * 2 * BN * 128 + 8 + 16 * FA_MAX_STAGES + 1024;
-  const int smem = 2 * FA_QTILE + fp.stages * 2 * BN * 128 + 8 + 16 * FA_MAX_STAGES + 1024;
+  constexpr int bars = 8 + 4 * 8 * FA_MAX_STAGES;
+  constexpr int smem_max = NC * FA_QTILE + FA_MAX_STAGES * 2 * BN * 128 + bars + 1024;
+  const int smem = NC * FA_QTILE + fp.stages * 2 * BN * 128 + bars + 1024;
   static bool attr_done[HI3D_MAX_DEVICES];
-  if (ensure_dyn_smem(fmha_tc5_kernel<BN>, smem_max, attr_done, "hi3d_attention_d64_tc5")) return -1;
-  dim3 grid((fp.L + FA_BM - 1) / FA_BM, heads, n_img);
-  fmha_tc5_kernel<BN><<<grid, FA_THREADS, smem, st>>>(fp);
+  if (ensure_dyn_smem(fmha_tc5_kernel<BN, NC, EMU8>, smem_max, attr_done, "hi3d_attention_d64_tc5")) return -1;
+  dim3 grid((fp.L + 64 * NC - 1) / (64 * NC), heads, n_img);
+  fmha_tc5_kernel<BN, NC, EMU8><<<grid, 128 * (NC + 1), smem, st>>>(fp);
   return check_launch("hi3d_attention_d64_tc5");
+}
+
+template <int EMU8>
+static int launch_variant(FaParams& fp, const void* qkv, int n_img, int heads, cudaStream_t st) {
+  const int bn = FA_VARIANT_BN[g_variant], nc = FA_VARIANT_NC[g_variant];
+  if (bn == 128) return launch_fmha<128, 2, EMU8>(fp, qkv, n_img, heads, st);
+  return nc == 3 ? launch_fmha<64, 3, EMU8>(fp, qkv, n_img, heads, st) : launch_fmha<64, 2, EMU8>(fp, qkv, n_img, heads, st);
 }
 
 }  // namespace hi3d
@@ -248,11 +346,20 @@ extern "C" int hi3d_attention_d64_tc5(const void* qkv, int n_img, int L, int hea
   fp.L = L;
   fp.C = heads * 64;
   fp.stages = FA_VARIANT_STAGES[g_variant];
-  fp.emu8 = g_emu <= 4 ? 2 * g_emu : (g_emu == 5 ? 3 : (g_emu == 6 ? 1 : 5));
   fp.scale_log2 = scale * 1.4426950408889634f;
   fp.out = (__half*)out;
   const cudaStream_t st = (cudaStream_t)stream;
-  return FA_VARIANT_BN[g_variant] == 128 ? launch_fmha<128>(fp, qkv, n_img, heads, st) : launch_fmha<64>(fp, qkv, n_img, heads, st);
+  const int emu8 = g_emu <= 4 ? 2 * g_emu : (g_emu == 5 ? 3 : (g_emu == 6 ? 1 : 5));
+  switch (emu8) {
+    case 0: return launch_variant<0>(fp, qkv, n_img, heads, st);
+    case 1: return launch_variant<1>(fp, qkv, n_img, heads, st);
+    case 2: return launch_variant<2>(fp, qkv, n_img, heads, st);
+    case 3: return launch_variant<3>(fp, qkv, n_img, heads, st);
+    case 4: return launch_variant<4>(fp, qkv, n_img, heads, st);
+    case 5: return launch_variant<5>(fp, qkv, n_img, heads, st);
+    case 6: return launch_variant<6>(fp, qkv, n_img, heads, st);
+    default: return launch_variant<8>(fp, qkv, n_img, heads, st);
+  }
 }
 
 extern "C" int hi3d_attention_tc5_set_variant(int variant) {

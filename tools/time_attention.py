@@ -1,0 +1,126 @@
+#!/usr/bin/env python
+"""Time the d = 64 spatial attention kernel (hi3d_attention_d64_tc5) at the four stage-2 UNet shapes (32 images x L tokens
+x heads: 16384 x 5, 4096 x 10, 1024 x 20, 256 x 20).  Each measurement is CUDA events around as many back-to-back calls as
+fill --window seconds, after warm-up.  Several libraries (--lib, any build of libhi3d_b200.so with the same C signature,
+e.g. one built from an earlier commit) are timed in one process, alternating between them over --rounds rounds, so that
+clock and power drift hits them alike.  --variants / --emus sweep hi3d_attention_tc5_set_variant and
+hi3d_attention_tc5_set_exp_emulation; without them each library runs its own default.  Prints one JSON line with the
+card's name, power limit and max SM clock beside the times.
+
+    python tools/time_attention.py [--lib PATH ...] [--rounds 3] [--window 1.0] [--variants 0,6] [--emus 0,1]
+"""
+import argparse
+import ctypes as C
+import json
+import os
+import subprocess
+import sys
+
+import torch
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+SHAPES = {"ds1": (32, 16384, 5), "ds2": (32, 4096, 10), "ds4": (32, 1024, 20), "ds8": (32, 256, 20)}
+
+
+def card():
+    try:
+        return subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                              capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
+    except Exception as e:  # noqa: BLE001
+        return f"unknown ({e})"
+
+
+def load(path):
+    lib = C.CDLL(os.path.abspath(path))
+    lib.hi3d_attention_d64_tc5.restype = C.c_int
+    lib.hi3d_attention_d64_tc5.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_void_p]
+    for f in ("hi3d_attention_tc5_set_variant", "hi3d_attention_tc5_set_exp_emulation"):
+        getattr(lib, f).restype = C.c_int
+        getattr(lib, f).argtypes = [C.c_int]
+    lib.hi3d_last_error.restype = C.c_char_p
+    return lib
+
+
+def check(lib, rc, what):
+    if rc != 0:
+        raise RuntimeError(f"{what}: {lib.hi3d_last_error().decode()}")
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--lib", action="append", help="library to time (repeatable); default: this tree's build")
+    ap.add_argument("--rounds", type=int, default=3)
+    ap.add_argument("--window", type=float, default=1.0, help="seconds of calls per measurement")
+    ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--shapes", default=",".join(SHAPES))
+    ap.add_argument("--variants", help="comma-separated hi3d_attention_tc5_set_variant values")
+    ap.add_argument("--emus", help="comma-separated hi3d_attention_tc5_set_exp_emulation values")
+    a = ap.parse_args()
+    if not torch.cuda.is_available():
+        sys.exit("time_attention.py needs a CUDA device")
+    if not a.lib:
+        from hi3d_official_b200 import build
+        a.lib = [build.build()]
+    libs = [(p, load(p)) for p in a.lib]
+    variants = [int(v) for v in a.variants.split(",")] if a.variants else [None]
+    emus = [int(e) for e in a.emus.split(",")] if a.emus else [None]
+    configs = [(v, e) for v in variants for e in emus]
+    stream = torch.cuda.current_stream()
+    res = {"gpu": card(), "rounds": a.rounds, "window_s": a.window, "libs": a.lib, "results": []}
+
+    def setup(lib, cfg):
+        v, e = cfg
+        if v is not None:
+            check(lib, lib.hi3d_attention_tc5_set_variant(v), "set_variant")
+        if e is not None:
+            check(lib, lib.hi3d_attention_tc5_set_exp_emulation(e), "set_exp_emulation")
+
+    for name in a.shapes.split(","):
+        n_img, L, heads = SHAPES[name]
+        C_ = heads * 64
+        g = torch.Generator(device="cuda").manual_seed(1)
+        qkv = torch.randn(n_img * L, 3 * C_, device="cuda", generator=g).half()
+        out = torch.empty(n_img * L, C_, device="cuda", dtype=torch.float16)
+        flop = 4.0 * n_img * heads * L * L * 64
+
+        def call(lib):
+            check(lib, lib.hi3d_attention_d64_tc5(qkv.data_ptr(), n_img, L, heads, 0.125, out.data_ptr(),
+                                                  C.c_void_p(stream.cuda_stream)), "hi3d_attention_d64_tc5")
+
+        def timed(lib, n):
+            t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            t0.record()
+            for _ in range(n):
+                call(lib)
+            t1.record()
+            torch.cuda.synchronize()
+            return t0.elapsed_time(t1) / n
+
+        # warm-up and the call count of every (library, config): enough calls to fill the window
+        calls, times = {}, {}
+        for li, (_, lib) in enumerate(libs):
+            for cfg in configs:
+                setup(lib, cfg)
+                for _ in range(a.warmup):
+                    call(lib)
+                calls[li, cfg] = max(3, int(a.window * 1e3 / timed(lib, 3)) + 1)
+                times[li, cfg] = []
+        for _ in range(a.rounds):
+            for li, (_, lib) in enumerate(libs):
+                for cfg in configs:
+                    setup(lib, cfg)
+                    times[li, cfg].append(timed(lib, calls[li, cfg]))
+        for (li, cfg), ts in times.items():
+            ms = sorted(ts)[len(ts) // 2]
+            res["results"].append({"shape": name, "n_img": n_img, "L": L, "heads": heads, "lib": li,
+                                   "variant": cfg[0], "emu": cfg[1], "calls": calls[li, cfg], "ms": round(ms, 4),
+                                   "ms_min": round(min(ts), 4), "ms_max": round(max(ts), 4),
+                                   "tflops": round(flop / ms / 1e9, 1)})
+        del qkv, out
+    print(json.dumps(res))
+
+
+if __name__ == "__main__":
+    main()
