@@ -13,7 +13,7 @@ from . import build as _build
 
 MAX_SEGS = 24
 ROWS_PLAIN, ROWS_CONV2D, ROWS_TEMPORAL = 0, 1, 2
-ACT_NONE, ACT_SILU, ACT_GEGLU, ACT_GELU, ACT_QUICKGELU = 0, 1, 2, 3, 4
+ACT_NONE, ACT_SILU, ACT_GEGLU, ACT_GELU, ACT_QUICKGELU, ACT_RELU = 0, 1, 2, 3, 4, 5
 
 
 class Hi3dError(RuntimeError):
@@ -102,6 +102,14 @@ _SIGS = {
                                     C.c_int, C.c_void_p]),
     "hi3d_clip_patchify": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                      C.c_void_p]),
+    "hi3d_dpt_stem_rows": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "hi3d_maxpool3x3s2_same": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "hi3d_groupnorm_apply_add": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                           C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int64, C.c_float, C.c_int, C.c_void_p,
+                                           C.c_int64, C.c_int64, C.c_void_p]),
+    "hi3d_upsample2x_bilinear_ac": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                              C.c_void_p]),
+    "hi3d_relu_copy": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     "hi3d_gaussian_sample": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
                                        C.c_float, C.c_void_p, C.c_void_p]),
     "hi3d_pack_weight": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,

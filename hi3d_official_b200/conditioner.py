@@ -8,12 +8,12 @@ that do not need third-party model weights, with the reference's names, ctor kwa
   DepthEmbedder                         vtdm/encoders.py:15-53   (resize, per-image min-max, 3x3 pixel-unshuffle to 9 channels)
   AesEmbedder                           vtdm/encoders.py:56-90   ([score | timestep_embedding(100 score, 255)])
 
-The image towers -- OpenCLIP ViT-H/14 (image embedding) and OpenAI CLIP ViT-L/14 + the aesthetic MLP (score) -- run natively on
-this package's kernels (clip_vision.py) once their weights are loaded: from the reference's files (the OpenCLIP embedder's
-`version` path; ckpts/ViT-L-14.pt and ckpts/metric_models/sac+logos+ava1-l14-linearMSE.pth relative to the working directory,
-as vtdm/encoders.py:60-64 hard-codes them), or from the `conditioner.embedders.N.*` tensors of a full checkpoint
-(GeneralConditioner.load_tower_weights, called by DiffusionEngine.init_from_ckpt), which win.  MiDaS DPT-hybrid (depth) stays a
-third-party network outside the H100 path.  Every tower sits behind an `ExternalTower`: a callable installed with
+The three towers -- OpenCLIP ViT-H/14 (image embedding), OpenAI CLIP ViT-L/14 + the aesthetic MLP (score) and MiDaS DPT-Hybrid
+(depth) -- run natively on this package's kernels (clip_vision.py, midas.py) once their weights are loaded: from the reference's
+files (the OpenCLIP embedder's `version` path; ckpts/ViT-L-14.pt, ckpts/metric_models/sac+logos+ava1-l14-linearMSE.pth and
+ckpts/dpt_hybrid_384.pt relative to the working directory, as vtdm/encoders.py:18,60-64 hard-codes them), or from the
+`conditioner.embedders.N.*` tensors of a full checkpoint (GeneralConditioner.load_tower_weights, called by
+DiffusionEngine.init_from_ckpt), which win.  Every tower sits behind an `ExternalTower`: a callable installed with
 `.set_fn(...)` comes first, then the native tower, and a pre-computed tensor passed in the batch under `<input_key>:<tower>`
 (e.g. batch["cond_frames_without_noise:clip"] = (B, 1024)) takes precedence over both.  Without weights, calling a tower
 raises.  Everything AROUND the towers is the reference's arithmetic, so the unmodified conditioner_config instantiates and
@@ -105,7 +105,33 @@ class FrozenOpenCLIPImageEmbedder(ExternalTower):
 
 
 class MiDaSInference(ExternalTower):
-    """annotator/midas/api.py:146-165 (DPT-hybrid -> (N, h, w) inverse depth)."""
+    """annotator/midas/api.py:146-165 (DPT-hybrid -> (N, h, w) inverse depth).  Native (midas.py) once weights are loaded: at
+    construction from ckpts/dpt_hybrid_384.pt under the working directory when it exists (the path vtdm/encoders.py:18
+    hard-codes), or later with load_weights()."""
+    PATH = os.path.join("ckpts", "dpt_hybrid_384.pt")
+
+    def __init__(self, *args, **kwargs):
+        super().__init__(*args, **kwargs)
+        self._sd: Optional[Dict[str, torch.Tensor]] = None       # the reference's DPTDepthModel tensors, packed on first use
+        self._tower = None
+        if os.path.isfile(self.PATH):
+            from . import midas
+            self.load_weights(midas.load_dpt_hybrid(self.PATH))
+
+    def load_weights(self, sd: Dict[str, torch.Tensor]):
+        """`sd`: the DPTDepthModel state dict (reference keys); raises KeyError when a tensor is missing."""
+        from . import midas
+        self._sd, self._tower = midas.live_state_dict(dict(sd)), None
+        return self
+
+    def native(self) -> Optional[Callable]:
+        return None if self._sd is None else self._run_native
+
+    def _run_native(self, x: torch.Tensor) -> torch.Tensor:
+        from . import midas
+        if self._tower is None or self._tower.device != x.device:
+            self._tower = midas.DPTHybridTower(self._sd, device=x.device)
+        return self._tower(x)
 
 
 class AestheticScore(ExternalTower):
@@ -235,7 +261,7 @@ def depth_to_concat(y: torch.Tensor, H: int, W: int, shuffle_size: int = 3) -> t
 
 
 class DepthEmbedder(AbstractEmbModel):
-    """vtdm/encoders.py:15-53 around an external depth estimator (`self.model`, MiDaS in the reference)."""
+    """vtdm/encoders.py:15-53 around the MiDaS DPT-Hybrid depth tower (`self.model`)."""
 
     def __init__(self, freeze: bool = True, use_3d: bool = False, shuffle_size: int = 3, scale_factor: float = 2.6666):
         super().__init__()
@@ -313,8 +339,9 @@ class GeneralConditioner(nn.Module):
 
     # -- native tower weights from a full checkpoint (DiffusionEngine.init_from_ckpt) ---------------------------------------------
     def load_tower_weights(self, sd: Dict[str, torch.Tensor], prefix: str = "conditioner.") -> List[str]:
-        """Routes `<prefix>embedders.N.open_clip.model.visual.*`, `...N.aesthetic_model.visual.*` and `...N.aesthetic_mlp.*` to the
-        native towers (the reference's module paths).  Returns the names of the towers that received weights."""
+        """Routes `<prefix>embedders.N.open_clip.model.visual.*`, `...N.aesthetic_model.visual.*`, `...N.aesthetic_mlp.*` and
+        `...N.model.model.*` (DepthEmbedder -> MiDaSInference -> DPTDepthModel) to the native towers (the reference's module paths).
+        Returns the names of the towers that received weights."""
         from . import clip_vision
         loaded = []
         for i, e in enumerate(self.embedders):
@@ -330,6 +357,11 @@ class GeneralConditioner(nn.Module):
                 if vis or mlp:
                     e.scorer.load_weights(vis or None, *(clip_vision.fold_linear_chain(mlp) if mlp else (None, None)))
                     loaded.append("aes")
+            elif isinstance(e, DepthEmbedder) and isinstance(e.model, MiDaSInference):
+                dpt = {k[len(p + "model.model."):]: v for k, v in sd.items() if k.startswith(p + "model.model.")}
+                if dpt:
+                    e.model.load_weights(dpt)
+                    loaded.append("depth")
         return loaded
 
     def missing_towers(self) -> List[str]:

@@ -106,10 +106,16 @@ struct alignas(16) Half8 {
   }
 };
 
-// HI3D_ACT_GELU / HI3D_ACT_QUICKGELU (the CLIP towers' MLP activations) on eight staged fp16 GEMM outputs.  Both GEMM
-// engines apply them in their store pass, on the fp16 tile, before the residual: the register pass that produces the tile
-// (bias, SiLU, GEGLU) is shared by every UNet GEMM, and code added to that unrolled loop slowed those GEMMs down.
-HI3D_DEVINL void clip_act_half8(int act, Half8& v) {
+// HI3D_ACT_GELU / HI3D_ACT_QUICKGELU (the CLIP towers' MLP activations) and HI3D_ACT_RELU (the DPT depth tower's convs) on
+// eight staged fp16 GEMM outputs.  Both GEMM engines apply them in their store pass, on the fp16 tile, before the residual:
+// the register pass that produces the tile (bias, SiLU, GEGLU) is shared by every UNet GEMM, and code added to that unrolled
+// loop slowed those GEMMs down.
+HI3D_DEVINL void store_act_half8(int act, Half8& v) {
+  if (act == HI3D_ACT_RELU) {
+#pragma unroll
+    for (int q = 0; q < 4; q++) v.h[q] = __hmax2_nan(v.h[q], __float2half2_rn(0.f));
+    return;
+  }
 #pragma unroll
   for (int q = 0; q < 4; q++) {
     float2 a = __half22float2(v.h[q]);

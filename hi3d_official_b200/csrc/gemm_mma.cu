@@ -264,7 +264,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 2) gemm_mma_kernel(const __grid_
       mo = ((long long)n_ * 2 * p.Ho + 2 * y_ + p.out_py) * (2 * p.Wo) + 2 * x_ + p.out_px;
     }
     Half8 v = *reinterpret_cast<const Half8*>(sC + r * pitch + c * 8);
-    if (p.act >= HI3D_ACT_GELU) clip_act_half8(p.act, v);
+    if (p.act >= HI3D_ACT_GELU) store_act_half8(p.act, v);
     if (res != nullptr) {
       Half8 rr = *reinterpret_cast<const Half8*>(res + mo * p.res_ld + nc);
 #pragma unroll
@@ -321,7 +321,7 @@ int validate_gemm(const hi3d_gemm_params* p, const char* who) {
   if (p->blend_x && (((uintptr_t)p->blend_x & 15) || p->blend_ld % 8)) { set_error("%s: blend_x misaligned", who); return -2; }
   if (p->rowbias && (p->rb_div <= 0 || p->rb_mod <= 0 || p->rb_ld % 2)) { set_error("%s: bad rowbias div/mod/ld", who); return -2; }
   if (p->act == HI3D_ACT_GEGLU && (p->N % 16)) { set_error("%s: GEGLU needs N %% 16 == 0", who); return -2; }
-  if (p->act < HI3D_ACT_NONE || p->act > HI3D_ACT_QUICKGELU) { set_error("%s: unknown activation %d", who, p->act); return -2; }
+  if (p->act < HI3D_ACT_NONE || p->act > HI3D_ACT_RELU) { set_error("%s: unknown activation %d", who, p->act); return -2; }
   if (p->mode == HI3D_ROWS_CONV2D) {
     if (p->Ho <= 0 || p->Wo <= 0 || p->Hs <= 0 || p->Ws <= 0 || (p->stride != 1 && p->stride != 2) ||
         (p->ups != 0 && p->ups != 1) || (p->M % (p->Ho * p->Wo))) {
@@ -390,8 +390,8 @@ extern "C" int hi3d_gemm(const hi3d_gemm_params* p, void* stream) {
 
 extern "C" const char* hi3d_last_error(void) { return hi3d::g_err; }
 extern "C" int64_t hi3d_launch_count(void) { return (int64_t)hi3d::g_launches.load(); }
-// 2: hi3d_gemm_params gained gn_stats / gn_unit / gn_rows.  Still 2 with HI3D_ACT_GELU / HI3D_ACT_QUICKGELU, hi3d_attention_d80_tc5
-// and hi3d_clip_patchify: they are additions (the parameter block and every existing entry point are unchanged); _native.py
+// 2: hi3d_gemm_params gained gn_stats / gn_unit / gn_rows.  Still 2 with HI3D_ACT_GELU / HI3D_ACT_QUICKGELU, hi3d_attention_d80_tc5,
+// hi3d_clip_patchify, HI3D_ACT_RELU and the DPT kernels of dpt.cu: they are additions (the parameter block and every existing entry point are unchanged); _native.py
 // checks that each declared symbol is exported.
 extern "C" int hi3d_abi_version(void) { return 2; }
 

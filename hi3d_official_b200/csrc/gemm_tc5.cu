@@ -257,7 +257,7 @@ __global__ void __launch_bounds__(128 + 256 * NT, 1) gemm_tc5_kernel(const __gri
       mo = ((long long)n_ * 2 * p.Ho + 2 * y_ + p.out_py) * (2 * p.Wo) + 2 * x_ + p.out_px;
     }
     Half8 v = *reinterpret_cast<const Half8*>(sC + r * pitch + c * 8);
-    if (p.act >= HI3D_ACT_GELU) clip_act_half8(p.act, v);
+    if (p.act >= HI3D_ACT_GELU) store_act_half8(p.act, v);
     if (p.residual != nullptr) {
       const Half8 rr = *reinterpret_cast<const Half8*>(p.residual + mo * p.res_ld + nc);
 #pragma unroll

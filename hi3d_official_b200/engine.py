@@ -4,9 +4,9 @@ vtdm/vtdm_gen_v01.py / vtdm/vtdm_gen_stage2_degradeImage.py, restricted to what 
 reference's key prefixes, `encode_first_stage` / `decode_first_stage`, `.denoiser/.model/.sampler/.conditioner`
 attributes, and the two hot loops (`sample_stage1`, `sample_stage2`) restated on top of the fused sampler.
 
-Out of scope (SURVEY.md section 2): training (`shared_step`, optimisers, EMA, logging) and the MiDaS depth tower.  The CLIP
-image towers run natively (clip_vision.py); `init_from_ckpt` hands their `conditioner.embedders.N.*` tensors to the
-conditioner.  `PassThroughConditioner` keeps the seam: it returns conditioning dictionaries that the caller supplies
+Out of scope (SURVEY.md section 2): training (`shared_step`, optimisers, EMA, logging).  The conditioner's towers -- the CLIP
+image towers and the MiDaS DPT-Hybrid depth tower -- run natively (clip_vision.py, midas.py); `init_from_ckpt` hands their
+`conditioner.embedders.N.*` tensors to the conditioner.  `PassThroughConditioner` keeps the seam: it returns conditioning dictionaries that the caller supplies
 pre-computed (synthetic in the benches).
 """
 from __future__ import annotations

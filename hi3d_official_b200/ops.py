@@ -12,7 +12,8 @@ from typing import List, Optional, Sequence, Tuple
 import torch
 
 from . import _native as N
-from ._native import ACT_GEGLU, ACT_GELU, ACT_NONE, ACT_QUICKGELU, ACT_SILU, ROWS_CONV2D, ROWS_PLAIN, ROWS_TEMPORAL  # noqa: F401
+from ._native import (ACT_GEGLU, ACT_GELU, ACT_NONE, ACT_QUICKGELU, ACT_RELU, ACT_SILU, ROWS_CONV2D, ROWS_PLAIN,  # noqa: F401
+                      ROWS_TEMPORAL)
 
 F16 = torch.float16
 
@@ -340,6 +341,79 @@ def clip_patchify(img: torch.Tensor, patch: int, out: torch.Tensor, normalize: b
         raise ValueError(f"clip_patchify: out must be [{rows}, Kpad], got {tuple(out.shape)}")
     N.check(N.load().hi3d_clip_patchify(img.data_ptr(), int(img.dtype == torch.float32), n, h, w, patch, int(normalize),
                                         out.shape[1], out.data_ptr(), _stream()), "hi3d_clip_patchify")
+
+
+def dpt_stem_rows(img: torch.Tensor, out: torch.Tensor):
+    """img: contiguous NCHW [n, 3, H, W] fp32 / fp16 -> out fp16 [n * ceil(H/2) * ceil(W/2), Kpad]: the rows of BiT's 7x7
+    stride-2 "same" stem conv, K ordered (c, ky, kx) (hi3d_dpt_stem_rows)."""
+    if not img.is_cuda or not img.is_contiguous() or img.dtype not in (torch.float32, F16) or img.dim() != 4 or img.shape[1] != 3:
+        raise ValueError("dpt_stem_rows: contiguous CUDA fp32/fp16 NCHW [n, 3, H, W] expected")
+    _chk16(out, "out")
+    n, _, h, w = img.shape
+    rows = n * ((h + 1) // 2) * ((w + 1) // 2)
+    if out.dim() != 2 or out.shape[0] != rows:
+        raise ValueError(f"dpt_stem_rows: out must be [{rows}, Kpad], got {tuple(out.shape)}")
+    N.check(N.load().hi3d_dpt_stem_rows(img.data_ptr(), int(img.dtype == torch.float32), n, h, w, out.shape[1], out.data_ptr(),
+                                        _stream()), "hi3d_dpt_stem_rows")
+
+
+def maxpool3x3s2_same(x: torch.Tensor, n: int, H: int, W: int, y: torch.Tensor):
+    """x fp16 [n*H*W, C] -> y fp16 [n*ceil(H/2)*ceil(W/2), C] (hi3d_maxpool3x3s2_same)."""
+    _chk16(x, "x"); _chk16(y, "y")
+    C_ = x.shape[-1]
+    if x.numel() != n * H * W * C_ or y.shape[-1] != C_ or y.numel() != n * ((H + 1) // 2) * ((W + 1) // 2) * C_:
+        raise ValueError(f"maxpool3x3s2_same: x {tuple(x.shape)} / y {tuple(y.shape)} do not fit {n} x {H} x {W}")
+    N.check(N.load().hi3d_maxpool3x3s2_same(x.data_ptr(), n, H, W, C_, y.data_ptr(), _stream()), "hi3d_maxpool3x3s2_same")
+
+
+def groupnorm_apply_add(x: torch.Tensor, stats: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, unit: int, n_images: int,
+                        y: torch.Tensor, add: Optional[torch.Tensor] = None, add_stats: Optional[torch.Tensor] = None,
+                        add_gamma: Optional[torch.Tensor] = None, add_beta: Optional[torch.Tensor] = None, relu: bool = False,
+                        eps: float = 1e-5, y_sample_rows: int = 0, y_row_off: int = 0):
+    """y = [relu](GroupNorm32(x) + add | GroupNorm32(add) | 0), statistics from the GEMM epilogue tables (hi3d_groupnorm_apply_add).
+    x / add fp16 [n_images * rows, C]; stats / add_stats fp32 [n_images, C / unit, 2]."""
+    _chk16(x, "x"); _chk16(y, "y"); _chk32(stats, "stats"); _chk32(gamma, "gamma"); _chk32(beta, "beta")
+    C_ = x.shape[-1]
+    rows = x.numel() // C_ // n_images
+    if rows * n_images * C_ != x.numel() or y.shape[-1] != C_ or stats.numel() < n_images * (C_ // unit) * 2:
+        raise ValueError(f"groupnorm_apply_add: x {tuple(x.shape)}, y {tuple(y.shape)}, stats {tuple(stats.shape)} do not fit "
+                         f"{n_images} images, unit {unit}")
+    if y.numel() < ((n_images - 1) * y_sample_rows + y_row_off + rows if y_sample_rows else n_images * rows) * C_:
+        raise ValueError("groupnorm_apply_add: y too small")
+    if add is not None:
+        _chk16(add, "add")
+        if add.shape != x.shape:
+            raise ValueError("groupnorm_apply_add: add must have x's shape")
+    if add_stats is not None:
+        _chk32(add_stats, "add_stats"); _chk32(add_gamma, "add_gamma"); _chk32(add_beta, "add_beta")
+        if add_stats.numel() < n_images * (C_ // unit) * 2:
+            raise ValueError("groupnorm_apply_add: add_stats too small")
+    N.check(N.load().hi3d_groupnorm_apply_add(x.data_ptr(), stats.data_ptr(), gamma.data_ptr(), beta.data_ptr(), _ptr(add),
+                                              _ptr(add_stats), _ptr(add_gamma), _ptr(add_beta), C_, unit, n_images, rows, eps,
+                                              int(relu), y.data_ptr(), y_sample_rows, y_row_off, _stream()),
+            "hi3d_groupnorm_apply_add")
+
+
+def upsample2x_bilinear_ac(x: torch.Tensor, n: int, H: int, W: int, y: torch.Tensor, add: Optional[torch.Tensor] = None):
+    """x fp16 [n*H*W, C] -> y fp16 [n*2H*2W, C] = bilinear x2 with align_corners=True (+ add) (hi3d_upsample2x_bilinear_ac)."""
+    _chk16(x, "x"); _chk16(y, "y")
+    C_ = x.shape[-1]
+    if x.numel() != n * H * W * C_ or y.shape[-1] != C_ or y.numel() != 4 * n * H * W * C_:
+        raise ValueError(f"upsample2x_bilinear_ac: x {tuple(x.shape)} / y {tuple(y.shape)} do not fit {n} x {H} x {W}")
+    if add is not None:
+        _chk16(add, "add")
+        if add.shape != y.shape:
+            raise ValueError("upsample2x_bilinear_ac: add must have y's shape")
+    N.check(N.load().hi3d_upsample2x_bilinear_ac(x.data_ptr(), n, H, W, C_, _ptr(add), y.data_ptr(), _stream()),
+            "hi3d_upsample2x_bilinear_ac")
+
+
+def relu_copy(x: torch.Tensor, y: torch.Tensor):
+    """y = max(x, 0), fp16 tensors of equal size (hi3d_relu_copy)."""
+    _chk16(x, "x"); _chk16(y, "y")
+    if x.numel() != y.numel():
+        raise ValueError("relu_copy: size mismatch")
+    N.check(N.load().hi3d_relu_copy(x.data_ptr(), x.numel(), y.data_ptr(), _stream()), "hi3d_relu_copy")
 
 
 def gaussian_sample(moments: torch.Tensor, noise: Optional[torch.Tensor], out: torch.Tensor, scale: float):

@@ -60,9 +60,10 @@ typedef struct {
 } hi3d_seg;
 
 enum { HI3D_ROWS_PLAIN = 0, HI3D_ROWS_CONV2D = 1, HI3D_ROWS_TEMPORAL = 2 };
-/* GELU: exact erf GELU (nn.GELU, open_clip ViT-H MLP); QUICKGELU: x*sigmoid(1.702x) (OpenAI CLIP clip/model.py MLP).  Both are
+/* GELU: exact erf GELU (nn.GELU, open_clip ViT-H MLP); QUICKGELU: x*sigmoid(1.702x) (OpenAI CLIP clip/model.py MLP); RELU:
+ * max(x, 0) (the MiDaS DPT head and residual conv units, annotator/midas/blocks.py, dpt_depth.py:89-96).  All three are
  * applied in fp32 to the fp16-rounded value (+ bias) in the epilogue's store pass, before the residual add. */
-enum { HI3D_ACT_NONE = 0, HI3D_ACT_SILU = 1, HI3D_ACT_GEGLU = 2, HI3D_ACT_GELU = 3, HI3D_ACT_QUICKGELU = 4 };
+enum { HI3D_ACT_NONE = 0, HI3D_ACT_SILU = 1, HI3D_ACT_GEGLU = 2, HI3D_ACT_GELU = 3, HI3D_ACT_QUICKGELU = 4, HI3D_ACT_RELU = 5 };
 
 typedef struct {
   int32_t M, N, K;          /* K == sum of seg[i].C; N multiple of 8                                   */
@@ -279,6 +280,37 @@ int hi3d_nhwc_to_nchw(const void* in, int in_ld, int N, int C, int H, int W, flo
  * in raster order, K ordered (c, ky, kx), columns >= 3*patch*patch zero.  Kpad: multiple of 8. */
 int hi3d_clip_patchify(const void* img, int img_is_fp32, int n, int H, int W, int patch, int normalize, int Kpad, void* out,
                        void* stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * MiDaS DPT-Hybrid depth tower (annotator/midas/{dpt_depth,vit,blocks}.py, timm vit_base_resnet50_384; hi3d_official_b200/midas.py).
+ * Its convs and linears are hi3d_gemm_tc5 calls; these kernels do what the GEMM epilogues cannot.
+ * --------------------------------------------------------------------------------------------- */
+/* Patch rows of BiT's 7x7 stride-2 stem conv with TF "same" zero padding (timm StdConv2dSame: before the first row
+ * ((ceil(H/2) - 1) * 2 + 7 - H) / 2, i.e. 2 for even H; columns alike), for one plain GEMM against the standardised
+ * weight.reshape(Co, 147) zero-padded to Kpad columns.  img: NCHW [n, 3, H, W] fp32 or fp16; out: fp16
+ * [n * ceil(H/2) * ceil(W/2), Kpad], K ordered (c, ky, kx), columns >= 147 zero.  Kpad: multiple of 8, >= 147. */
+int hi3d_dpt_stem_rows(const void* img, int img_is_fp32, int n, int H, int W, int Kpad, void* out, void* stream);
+/* 3x3 stride-2 max-pool with TF "same" padding by -inf (timm MaxPool2dSame after the stem): x fp16 NHWC [n, H, W, C] ->
+ * y [n, ceil(H/2), ceil(W/2), C]; for even sizes the pad is one row / column after the image.  C multiple of 8. */
+int hi3d_maxpool3x3s2_same(const void* x, int n, int H, int W, int C, void* y, void* stream);
+/* y = [ReLU](GroupNorm32(x) + addend) in one pass, for the bottlenecks of BiT (timm ResNetV2 Bottleneck, preact=False:
+ * act3(norm3(conv3) + shortcut)) and its stem's GroupNorm + ReLU.  x fp16 [n_images * rows_per_image, C]; its group statistics
+ * come from `stats`, the hi3d_gemm_params::gn_stats table of the GEMM that wrote x (fp32 [n_images, C / unit, 2]); gamma /
+ * beta fp32 [C].  The addend is NULL, a raw fp16 tensor of x's shape (add_stats NULL), or a second GroupNorm-affine tensor
+ * GroupNorm32(add) with its own table and parameters (the projection shortcut of a stage's first block).  Statistics are
+ * combined in fp64; the arithmetic is fp32 and y is rounded once.  y may be haloed: image i starts at row
+ * i * y_sample_rows + y_row_off (0, 0 = dense).  C multiple of 32 and 8, <= 2048; unit divides C / 32. */
+int hi3d_groupnorm_apply_add(const void* x, const float* stats, const float* gamma, const float* beta, const void* add,
+                             const float* add_stats, const float* add_gamma, const float* add_beta, int C, int unit, int n_images,
+                             int64_t rows_per_image, float eps, int apply_relu, void* y, int64_t y_sample_rows,
+                             int64_t y_row_off, void* stream);
+/* F.interpolate(scale_factor=2, mode='bilinear', align_corners=True) of the fusion blocks and the head (blocks.py
+ * FeatureFusionBlock_custom, Interpolate) on fp16 NHWC [n, H, W, C] -> y [n, 2H, 2W, C], plus an optional addend of y's shape
+ * (the next fusion block's xs[0] + resConfUnit1(xs[1])), in fp32 with one rounding.  C multiple of 8. */
+int hi3d_upsample2x_bilinear_ac(const void* x, int n, int H, int W, int C, const void* add, void* y, void* stream);
+/* y = max(x, 0) over n fp16 values (n multiple of 8): the ReLU that opens a residual conv unit (blocks.py
+ * ResidualConvUnit_custom), whose input x is still needed for the unit's residual. */
+int hi3d_relu_copy(const void* x, int64_t n, void* y, void* stream);
 
 /* DiagonalGaussianDistribution.sample / mode (distributions.py:24-41,71) * scale_factor (diffusion.py:149):
  * moments fp16 NHWC [N, H, W, ld] (mean = ch 0..C-1, logvar = ch C..2C-1), noise fp32 NCHW or NULL (mode),

@@ -3,9 +3,10 @@
 engine.  Reads <output_dir>/first_step/first.pt (stage-1 frames written by pipeline_i2v_eval_v01.py; first.mp4 through
 OpenCV when the tensor is absent, like v02:169-176), up-samples them to 1024^2, VAE-encodes each frame (posterior sample,
 CPU RNG like the reference), runs the 25-step re-noise/blend loop of pipeline_i2v_eval_v02.py:127-135 on the fused sampler,
-decodes and writes second_step_video/second.mp4.  Conditioning: --towers {'clip': (1,1024), 'depth': (T,h',w') MiDaS maps} /
---cond / --synthetic as in v01; 'clip' may be left out of --towers when the OpenCLIP tower's weights are available (it then
-runs natively in the conditioner; MiDaS depth always comes from --towers); --tiny = the smoke size the tests run."""
+decodes and writes second_step_video/second.mp4.  Conditioning, in v01's order: --cond, --towers {'clip': (1,1024), 'depth':
+(T,h',w') MiDaS maps}, --synthetic, and otherwise, when the OpenCLIP and MiDaS DPT-Hybrid towers have weights (their files under
+the working directory or their tensors in the checkpoint), the model's own conditioner builds c / uc from the frames.  A tower
+left out of --towers runs natively; --tiny = the smoke size the tests run."""
 import argparse
 import os
 import random
@@ -13,7 +14,7 @@ import random
 import torch
 import torch.nn.functional as F
 
-from pipeline_i2v_eval_v01 import cond_from_towers, load_model, save_frames, synthetic_cond
+from pipeline_i2v_eval_v01 import cond_from_towers, load_model, native_towers_ready, save_frames, synthetic_cond
 
 
 def main():
@@ -56,8 +57,11 @@ def main():
         c, uc = cond_from_towers(model, frames.permute(1, 0, 2, 3).contiguous(), torch.load(params.towers), params.elevation, 2)
     elif params.synthetic:
         c, uc = synthetic_cond(2, T, h, "cuda", seed)
+    elif native_towers_ready(model):
+        c, uc = cond_from_towers(model, frames.permute(1, 0, 2, 3).contiguous(), None, params.elevation, 2)
     else:
-        raise SystemExit("the conditioner towers are outside the H100 hot path: pass --towers / --cond <file> or --synthetic")
+        raise SystemExit(f"the conditioner's towers {model.conditioner.missing_towers()} have no weights: put their files under ckpts/ "
+                         f"(open_clip_pytorch_model.bin, dpt_hybrid_384.pt), or pass --towers / --cond <file> or --synthetic")
     with torch.no_grad():
         init_latents = torch.randn(T, 4, h, h, device="cuda")                                      # v02:93
         z = torch.cat([model.encode_first_stage(frames[t:t + 1].half()) for t in range(T)], 0)     # v02:96-101
