@@ -110,6 +110,11 @@ _SIGS = {
     "hi3d_upsample2x_bilinear_ac": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
                                               C.c_void_p]),
     "hi3d_relu_copy": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
+    "hi3d_maxpool2x2_ceil": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p]),
+    "hi3d_resize_bilinear": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int,
+                                       C.c_int, C.c_void_p]),
+    "hi3d_u2net_fuse_sides": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int),
+                                        C.c_int, C.c_float, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "hi3d_gaussian_sample": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
                                        C.c_float, C.c_void_p, C.c_void_p]),
     "hi3d_pack_weight": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,

@@ -50,14 +50,20 @@ class SegSpec:
         self.c_off, self.dy, self.dx, self.dt = c_off, dy, dx, dt
 
 
-def conv_taps(srcs: Sequence[torch.Tensor], pad_lo: int = 1, ksize: int = 3) -> List[SegSpec]:
+def conv_taps(srcs: Sequence, pad_lo: int = 1, ksize: int = 3, dilation: int = 1) -> List[SegSpec]:
     """Segments of a kxk conv over the channel-concat of `srcs`: tap-major, source-minor -- the K order of
-    weight.permute(0, 2, 3, 1) of a conv whose input channels are [srcs[0] | srcs[1] | ...]."""
+    weight.permute(0, 2, 3, 1) of a conv whose input channels are [srcs[0] | srcs[1] | ...].  A source is a tensor or a
+    SegSpec (a channel range of a wider tensor).  Tap (ky, kx) reads offset ((ky - pad_lo) * dilation, (kx - pad_lo) * dilation):
+    with pad_lo = 1 a 3x3 conv with padding = dilation (U^2-Net's dilated REBNCONV)."""
     segs = []
     for ky in range(ksize):
         for kx in range(ksize):
+            dy, dx = (ky - pad_lo) * dilation, (kx - pad_lo) * dilation
             for s in srcs:
-                segs.append(SegSpec(s, dy=ky - pad_lo, dx=kx - pad_lo))
+                if isinstance(s, SegSpec):
+                    segs.append(SegSpec(s.src, C_=s.C, c_off=s.c_off, ld=s.ld, dy=dy, dx=dx))
+                else:
+                    segs.append(SegSpec(s, dy=dy, dx=dx))
     return segs
 
 
@@ -73,8 +79,15 @@ class Gemm:
                  rowbias: Optional[torch.Tensor] = None, rb_div: int = 1, rb_mod: int = 1, act: int = ACT_NONE,
                  residual: Optional[torch.Tensor] = None, blend_x: Optional[torch.Tensor] = None, alpha: float = 0.0,
                  engine: str = "mma", gn_stats: Optional[torch.Tensor] = None, gn_unit: int = 0, gn_rows: int = 0):
+        if out.is_contiguous():
+            _chk16(out, "out")
+            out_ld, out_rows = out.shape[-1], out.numel() // out.shape[-1]
+        else:                       # a column slice of a wider matrix (a channel slice of a concat buffer): rows of stride out_ld
+            if out.dtype != F16 or not out.is_cuda or out.dim() != 2 or out.stride(1) != 1:
+                raise ValueError(f"out: expected a contiguous CUDA fp16 tensor or a column slice of one, got {out.dtype} "
+                                 f"{out.device} {tuple(out.shape)} strides {out.stride()}")
+            out_ld, out_rows = out.stride(0), out.shape[0]
         _chk16(W, "W")
-        _chk16(out, "out")
         Nn, K = W.shape
         if len(segs) > N.MAX_SEGS:
             raise ValueError(f"too many segments ({len(segs)})")
@@ -112,8 +125,8 @@ class Gemm:
             _chk16(blend_x, "blend_x")
             p.blend_ld = blend_x.shape[-1]
         p.blend_x, p.alpha = _ptr(blend_x), float(alpha)
-        p.out, p.out_ld = out.data_ptr(), out.shape[-1]
-        if out.shape[-1] < n_out or out.numel() < M * out.shape[-1] * (4 if p.out_up else 1):
+        p.out, p.out_ld = out.data_ptr(), out_ld
+        if out.shape[-1] < n_out or out_rows < M * (4 if p.out_up else 1):
             raise ValueError(f"out too small: {tuple(out.shape)} for M={M} N_out={n_out}")
         if gn_stats is not None:      # GroupNorm statistics of the output from the epilogue (hi3d_gemm_params::gn_stats)
             _chk32(gn_stats, "gn_stats")
@@ -414,6 +427,51 @@ def relu_copy(x: torch.Tensor, y: torch.Tensor):
     if x.numel() != y.numel():
         raise ValueError("relu_copy: size mismatch")
     N.check(N.load().hi3d_relu_copy(x.data_ptr(), x.numel(), y.data_ptr(), _stream()), "hi3d_relu_copy")
+
+
+def _cols16(t: torch.Tensor, name: str) -> Tuple[int, int]:
+    """(pointer, row stride) of an fp16 matrix [rows, C] that may be a column slice of a wider one."""
+    if t.dtype != F16 or not t.is_cuda or t.dim() != 2 or t.stride(1) != 1:
+        raise ValueError(f"{name}: expected a CUDA fp16 matrix [rows, C] with unit column stride, got {t.dtype} {t.device} "
+                         f"{tuple(t.shape)} strides {t.stride()}")
+    return t.data_ptr(), t.stride(0)
+
+
+def maxpool2x2_ceil(x: torch.Tensor, n: int, H: int, W: int, y: torch.Tensor):
+    """MaxPool2d(2, 2, ceil_mode=True): x fp16 [n*H*W, C] -> y fp16 [n*ceil(H/2)*ceil(W/2), C]; either may be a column slice of a
+    wider matrix (hi3d_maxpool2x2_ceil)."""
+    (xp, xld), (yp, yld) = _cols16(x, "x"), _cols16(y, "y")
+    C_ = x.shape[1]
+    if x.shape[0] != n * H * W or y.shape != (n * ((H + 1) // 2) * ((W + 1) // 2), C_):
+        raise ValueError(f"maxpool2x2_ceil: x {tuple(x.shape)} / y {tuple(y.shape)} do not fit {n} x {H} x {W}")
+    N.check(N.load().hi3d_maxpool2x2_ceil(xp, xld, n, H, W, C_, yp, yld, _stream()), "hi3d_maxpool2x2_ceil")
+
+
+def resize_bilinear(x: torch.Tensor, n: int, Hs: int, Ws: int, y: torch.Tensor, Ht: int, Wt: int):
+    """F.interpolate(size=(Ht, Wt), mode='bilinear', align_corners=False): x fp16 [n*Hs*Ws, C] -> y fp16 [n*Ht*Wt, C]; either may
+    be a column slice of a wider matrix (hi3d_resize_bilinear)."""
+    (xp, xld), (yp, yld) = _cols16(x, "x"), _cols16(y, "y")
+    C_ = x.shape[1]
+    if x.shape[0] != n * Hs * Ws or y.shape != (n * Ht * Wt, C_):
+        raise ValueError(f"resize_bilinear: x {tuple(x.shape)} / y {tuple(y.shape)} do not fit {n} x {Hs}x{Ws} -> {Ht}x{Wt}")
+    N.check(N.load().hi3d_resize_bilinear(xp, xld, n, Hs, Ws, C_, yp, yld, Ht, Wt, _stream()), "hi3d_resize_bilinear")
+
+
+def u2net_fuse_sides(sides: Sequence[Tuple[torch.Tensor, int, int]], b0: float, n: int, H: int, W: int, out: torch.Tensor):
+    """out fp32 [n, H, W] = sigmoid(b0 + sum_k resize(side_k -> H x W)); sides = [(fp16 [n*h_k*w_k, ld_k] (channel 0 read), h_k,
+    w_k), ...], at most 8 (hi3d_u2net_fuse_sides)."""
+    _chk32(out, "out")
+    if out.numel() != n * H * W or not 1 <= len(sides) <= 8:
+        raise ValueError(f"u2net_fuse_sides: out {tuple(out.shape)} for {n} x {H} x {W}, {len(sides)} sides")
+    k = len(sides)
+    ptrs, lds, hs, ws = (C.c_void_p * k)(), (C.c_int * k)(), (C.c_int * k)(), (C.c_int * k)()
+    for i, (s, h, w) in enumerate(sides):
+        ptrs[i], lds[i] = _cols16(s, f"side {i}")
+        if s.shape[0] != n * h * w:
+            raise ValueError(f"u2net_fuse_sides: side {i} {tuple(s.shape)} does not fit {n} x {h} x {w}")
+        hs[i], ws[i] = h, w
+    N.check(N.load().hi3d_u2net_fuse_sides(ptrs, lds, hs, ws, k, float(b0), n, H, W, out.data_ptr(), _stream()),
+            "hi3d_u2net_fuse_sides")
 
 
 def gaussian_sample(moments: torch.Tensor, noise: Optional[torch.Tensor], out: torch.Tensor, scale: float):

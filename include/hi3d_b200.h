@@ -312,6 +312,25 @@ int hi3d_upsample2x_bilinear_ac(const void* x, int n, int H, int W, int C, const
  * ResidualConvUnit_custom), whose input x is still needed for the unit's residual. */
 int hi3d_relu_copy(const void* x, int64_t n, void* y, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * U^2-Net background removal (U-2-Net model/u2net.py, the default network of rembg's `remove`; hi3d_official_b200/u2net.py).
+ * Its convs (3x3, dilations 1 / 2 / 4 / 8, BatchNorm folded, ReLU epilogue, the RSU's `+ hxin` as the residual epilogue) are
+ * hi3d_gemm_tc5 calls; these kernels do the rest.  x_ld / y_ld are the channel strides of source and destination, so either
+ * may be a channel slice of a wider (concat) buffer: pass the slice's first element.  C, x_ld, y_ld multiples of 8.
+ * --------------------------------------------------------------------------------------------- */
+/* nn.MaxPool2d(2, 2, ceil_mode=True) (RSU pool1..pool5, U2NET pool12..pool56): fp16 NHWC [n, H, W, C] -> [n, ceil(H/2),
+ * ceil(W/2), C]; a window over the bottom / right edge takes the max of its valid elements. */
+int hi3d_maxpool2x2_ceil(const void* x, int x_ld, int n, int H, int W, int C, void* y, int y_ld, void* stream);
+/* F.interpolate(size=(Ht, Wt), mode='bilinear', align_corners=False) (u2net.py _upsample_like): fp16 NHWC [n, Hs, Ws, C] ->
+ * [n, Ht, Wt, C], any sizes.  Source coordinate max(0, (dst + 0.5) * Hs / Ht - 0.5) with Hs / Ht and the fused multiply-add in
+ * fp32; the blend in fp32 with one rounding. */
+int hi3d_resize_bilinear(const void* x, int x_ld, int n, int Hs, int Ws, int C, void* y, int y_ld, int Ht, int Wt, void* stream);
+/* Output 0 of U2NET.forward, sigmoid(outconv(cat(d1..d6))) with every d_k upsampled to H x W, when outconv's weights are folded
+ * into the side heads: out = sigmoid(b0 + sum_k resize(side_k)), fp32 [n, H, W].  sides[k]: fp16 NHWC [n, side_h[k],
+ * side_w[k], side_ld[k]], channel 0 read; the arrays are host memory of n_sides (<= 8) entries. */
+int hi3d_u2net_fuse_sides(const void* const* sides, const int* side_ld, const int* side_h, const int* side_w, int n_sides, float b0,
+                          int n, int H, int W, float* out, void* stream);
+
 /* DiagonalGaussianDistribution.sample / mode (distributions.py:24-41,71) * scale_factor (diffusion.py:149):
  * moments fp16 NHWC [N, H, W, ld] (mean = ch 0..C-1, logvar = ch C..2C-1), noise fp32 NCHW or NULL (mode),
  * out fp32 NCHW [N, C, H, W]. */

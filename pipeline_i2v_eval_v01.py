@@ -88,6 +88,28 @@ def load_image(path, size):
     return torch.from_numpy(np.ascontiguousarray(img)).permute(2, 0, 1).float() / 127.5 - 1.0
 
 
+def remove_background(image_path, output_dir):
+    """v01:153-168: rembg.remove with U^2-Net (hi3d_official_b200/rembg.py, weights ckpts/u2net.pth under the working directory),
+    the cut-out saved as <output_dir>/temp_image/rgba.png and pasted onto white through its alpha as temp_image/white.png, at
+    the input's size.  Returns the image stage 1 reads: white.png, or `image_path` itself when ckpts/u2net.pth is absent."""
+    from PIL import Image
+    from hi3d_official_b200 import rembg
+    if not os.path.exists(rembg.DEFAULT_WEIGHTS):
+        print(f"[hi3d-b200] WARNING: {rembg.DEFAULT_WEIGHTS} not found, background removal SKIPPED: stage 1 conditions on "
+              f"{image_path} as given, background included", flush=True)
+        return image_path
+    image = rembg.remove(Image.open(image_path), session=rembg.new_session())
+    temp_dir = os.path.join(output_dir, "temp_image")
+    os.makedirs(temp_dir, exist_ok=True)
+    image.save(os.path.join(temp_dir, "rgba.png"))
+    white_path = os.path.join(temp_dir, "white.png")
+    white = Image.new("RGB", image.size, "WHITE")
+    white.paste(image, mask=image.split()[3])
+    white.save(white_path)
+    print(f"[hi3d-b200] removed the background of {image_path}: {white_path}", flush=True)
+    return white_path
+
+
 def cond_from_towers(model, frames, towers, elevation, stage):
     """v01:62-78 / v02:104-118: batch -> add_custom_cond -> GeneralConditioner with the third-party towers' outputs supplied.
     frames: (3, T, H, W) in [-1, 1] on the GPU (stage 1: the image repeated T times)."""
@@ -135,12 +157,12 @@ def main():
         d = torch.load(params.cond, map_location="cuda")
         c, uc = d["c"], d["uc"]
     elif params.towers:
-        img = load_image(params.image_path, 8 * h).cuda()
+        img = load_image(remove_background(params.image_path, params.output_dir), 8 * h).cuda()
         c, uc = cond_from_towers(model, img[:, None].repeat(1, T, 1, 1), torch.load(params.towers), params.elevation, 1)
     elif params.synthetic:
         c, uc = synthetic_cond(1, T, h, "cuda", seed)
     elif native_towers_ready(model):
-        img = load_image(params.image_path, 8 * h).cuda()
+        img = load_image(remove_background(params.image_path, params.output_dir), 8 * h).cuda()
         c, uc = cond_from_towers(model, img[:, None].repeat(1, T, 1, 1), None, params.elevation, 1)
     else:
         raise SystemExit("the conditioner towers are outside the H100 hot path: pass --towers / --cond <file> or --synthetic")

@@ -17,6 +17,21 @@ import torch.nn.functional as F
 from pipeline_i2v_eval_v01 import cond_from_towers, load_model, native_towers_ready, save_frames, synthetic_cond
 
 
+def replace_first_frame(frames, output_dir, size):
+    """v02:184-188: frame 0 of the stage-1 video becomes the cut-out input <output_dir>/temp_image/white.png (written by
+    pipeline_i2v_eval_v01.py) -- cv2.imread, cv2.resize to size x size (INTER_LINEAR), BGR -> RGB, [-1, 1] -- when that file
+    exists.  frames: (T, 3, size, size) in [-1, 1], changed in place.  Returns whether frame 0 was replaced."""
+    import cv2
+    import numpy as np
+    path = os.path.join(output_dir, "temp_image", "white.png")
+    if not os.path.exists(path):
+        return False
+    img = cv2.cvtColor(cv2.resize(cv2.imread(path), [size, size]), cv2.COLOR_BGR2RGB)
+    frames[0] = (torch.from_numpy(np.ascontiguousarray(img)).permute(2, 0, 1).float() / 255.0 - 0.5) * 2.0
+    print(f"[hi3d-b200] frame 0 replaced by {path}", flush=True)
+    return True
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--denoise_config", type=str, default="configs/inference-v02.yaml")
@@ -50,6 +65,7 @@ def main():
         frames = torch.rand(T, 3, 8 * h, 8 * h, device="cuda") * 2 - 1
     else:
         raise SystemExit(f"{first} not found (run pipeline_i2v_eval_v01.py first) and --synthetic not given")
+    replace_first_frame(frames, params.output_dir, 8 * h)
     if params.cond:
         d = torch.load(params.cond, map_location="cuda")
         c, uc = d["c"], d["uc"]
