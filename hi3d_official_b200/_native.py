@@ -51,14 +51,6 @@ _SIGS = {
     "hi3d_gemm_tc5": (C.c_int, [C.POINTER(GemmParams), C.c_void_p]),
     "hi3d_gemm_tc5_set_pair_mode": (C.c_int, [C.c_int]),
     "hi3d_gemm_tc5_set_epilogue_warps": (C.c_int, [C.c_int]),
-    "hi3d_groupnorm_ws_floats": (C.c_int64, [C.c_int]),
-    "hi3d_groupnorm_silu": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_void_p,
-                                      C.c_void_p, C.c_float, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
-    "hi3d_groupnorm_sums": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_void_p, C.c_void_p,
-                                      C.c_void_p]),
-    "hi3d_groupnorm_apply": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_void_p, C.c_int64,
-                                       C.c_void_p, C.c_void_p, C.c_float, C.c_int, C.c_void_p, C.c_int64, C.c_int64,
-                                       C.c_void_p]),
     "hi3d_groupnorm_apply_stats": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int,
                                              C.c_int64, C.c_int, C.c_int64, C.c_void_p, C.c_void_p, C.c_float, C.c_int,
                                              C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
@@ -148,7 +140,7 @@ def load(build_if_missing: bool = True):
         fn = getattr(lib, name)   # AttributeError if the .so does not export a declared symbol
         fn.restype = res
         fn.argtypes = args
-    if lib.hi3d_abi_version() != 2:
+    if lib.hi3d_abi_version() != 3:
         raise Hi3dError("libhi3d_b200.so ABI version mismatch")
     _lib = lib
     return lib

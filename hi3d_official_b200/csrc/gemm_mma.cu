@@ -393,7 +393,9 @@ extern "C" int64_t hi3d_launch_count(void) { return (int64_t)hi3d::g_launches.lo
 // 2: hi3d_gemm_params gained gn_stats / gn_unit / gn_rows.  Still 2 with HI3D_ACT_GELU / HI3D_ACT_QUICKGELU, hi3d_attention_d80_tc5,
 // hi3d_clip_patchify, HI3D_ACT_RELU and the DPT kernels of dpt.cu: they are additions (the parameter block and every existing entry point are unchanged); _native.py
 // checks that each declared symbol is exported.
-extern "C" int hi3d_abi_version(void) { return 2; }
+// 3: GroupNorm statistics are unit tables only; the entry points of the chunked statistics pass, its workspace and the dense
+// apply over pre-reduced sums are removed.
+extern "C" int hi3d_abi_version(void) { return 3; }
 
 extern "C" int hi3d_device_info(int* sm_count, int* cc_major, int* cc_minor, int* max_smem_optin) {
   int dev = 0;

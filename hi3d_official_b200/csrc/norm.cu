@@ -7,7 +7,6 @@
 
 namespace hi3d {
 
-constexpr int GN_MAX_CHUNKS = 512;
 constexpr int GN_GROUPS = 32;
 constexpr int GN_UNROLL = 4;
 constexpr int GN_TARGET_CTAS = 132 * 4 * 4;   // ~4 waves at 4 CTAs/SM
@@ -22,95 +21,9 @@ HI3D_DEVINL Half8 ld_stream(const __half* p) {
   return v;
 }
 
-// ---- pass 1: per-(sample, chunk, group) partial sum / sum of squares -------------------------------
-// grid (chunks, n_samples); blockDim = RL * CV where CV = C/8 vector-columns.
-__global__ void __launch_bounds__(512)
-gn_stats_kernel(const __half* __restrict__ x1, int C1, const __half* __restrict__ x2, int C2, long long rows_per_sample,
-                long long rows_per_chunk, float* __restrict__ ws) {
-  __shared__ float sg[GN_GROUPS * 2];
-  const int C = C1 + C2, CV = C >> 3, cpg = C / GN_GROUPS;
-  const int tid = threadIdx.x;
-  if (tid < GN_GROUPS * 2) sg[tid] = 0.f;
-  __syncthreads();
-  const int cv = tid % CV, rl = tid / CV, RL = blockDim.x / CV;
-  const int n = blockIdx.y, chunk = blockIdx.x;
-  const long long r0 = (long long)chunk * rows_per_chunk;
-  long long r1 = r0 + rows_per_chunk;
-  if (r1 > rows_per_sample) r1 = rows_per_sample;
-  const int c0 = cv * 8;
-  const __half* base;
-  int ld;
-  if (c0 < C1) { base = x1 + c0; ld = C1; } else { base = x2 + (c0 - C1); ld = C2; }
-  base += (long long)n * rows_per_sample * ld;
-  float s[8], q[8];
-#pragma unroll
-  for (int e = 0; e < 8; e++) s[e] = q[e] = 0.f;
-  long long r = r0 + rl;
-  for (; r + (long long)(GN_UNROLL - 1) * RL < r1; r += (long long)GN_UNROLL * RL) {
-    Half8 v[GN_UNROLL];
-#pragma unroll
-    for (int u = 0; u < GN_UNROLL; u++) v[u] = ld_stream(base + (r + (long long)u * RL) * ld);
-#pragma unroll
-    for (int u = 0; u < GN_UNROLL; u++)
-#pragma unroll
-      for (int k = 0; k < 4; k++) {
-        const float2 f = __half22float2(v[u].h[k]);
-        s[2 * k] += f.x; q[2 * k] += f.x * f.x;
-        s[2 * k + 1] += f.y; q[2 * k + 1] += f.y * f.y;
-      }
-  }
-  for (; r < r1; r += RL) {
-    const Half8 v = ld_stream(base + r * ld);
-#pragma unroll
-    for (int k = 0; k < 4; k++) {
-      const float2 f = __half22float2(v.h[k]);
-      s[2 * k] += f.x; q[2 * k] += f.x * f.x;
-      s[2 * k + 1] += f.y; q[2 * k + 1] += f.y * f.y;
-    }
-  }
-  // fold the 8 channels into their groups (a vector may straddle a group boundary when cpg % 8 != 0)
-  int gcur = c0 / cpg;
-  float as = 0.f, aq = 0.f;
-#pragma unroll
-  for (int e = 0; e < 8; e++) {
-    const int gi = (c0 + e) / cpg;
-    if (gi != gcur) {
-      atomicAdd(&sg[2 * gcur], as); atomicAdd(&sg[2 * gcur + 1], aq);
-      as = aq = 0.f; gcur = gi;
-    }
-    as += s[e]; aq += q[e];
-  }
-  atomicAdd(&sg[2 * gcur], as); atomicAdd(&sg[2 * gcur + 1], aq);
-  __syncthreads();
-  if (tid < GN_GROUPS * 2) ws[((long long)n * GN_MAX_CHUNKS + chunk) * (GN_GROUPS * 2) + tid] = sg[tid];
-}
-
-// ---- pass 1b: combine the chunk partials of one sample into (sum, sum of squares) per group ----------------
-// grid (n_samples), 1024 threads; result at fin[n][32][2].  (Frame-sharded runs all-reduce `fin` across ranks here.)
-__global__ void __launch_bounds__(1024)
-gn_finalize_kernel(const float* __restrict__ ws, int nchunks, float* __restrict__ fin) {
-  __shared__ float stot[GN_GROUPS * 2];
-  const int tid = threadIdx.x, n = blockIdx.x;
-  if (tid < GN_GROUPS * 2) stot[tid] = 0.f;
-  __syncthreads();
-  const float* w = ws + (long long)n * GN_MAX_CHUNKS * (GN_GROUPS * 2);
-  // thread owns value index tid % 64 and chunks tid/64, +16, ...; 4 independent loads in flight per thread
-  float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
-  int c = tid >> 6;
-  for (; c + 48 < nchunks; c += 64) {
-    a0 += w[c * (GN_GROUPS * 2) + (tid & 63)];
-    a1 += w[(c + 16) * (GN_GROUPS * 2) + (tid & 63)];
-    a2 += w[(c + 32) * (GN_GROUPS * 2) + (tid & 63)];
-    a3 += w[(c + 48) * (GN_GROUPS * 2) + (tid & 63)];
-  }
-  for (; c < nchunks; c += 16) a0 += w[c * (GN_GROUPS * 2) + (tid & 63)];
-  atomicAdd(&stot[tid & 63], (a0 + a1) + (a2 + a3));
-  __syncthreads();
-  if (tid < GN_GROUPS * 2) fin[(long long)n * (GN_GROUPS * 2) + tid] = stot[tid];
-}
-
-// ---- pass 2: y = [silu]((x - mean) * rstd * gamma + beta) ------------------------------------------
-// grid (row_slabs, n_samples), blockDim = RL * CV.
+// ---- GroupNorm apply: y = [silu]((x - mean) * rstd * gamma + beta) ----------------------------------
+// grid (row_slabs, n_samples), blockDim = RL * CV.  Statistics: the unit tables stats1 / stats2 when stats1 != NULL, else the
+// per-(sample, group) sums `fin` over `count` elements.
 template <bool HALO>      // HALO = haloed output with peer stores / boundary zero fill (frame-sharded temporal GroupNorm only):
                           // a template so that the dense kernel keeps its 64 registers (2 CTAs per SM)
 __global__ void __launch_bounds__(512)
@@ -362,10 +275,6 @@ layernorm_generic_kernel(const __half* __restrict__ x, const __half* __restrict_
 
 using namespace hi3d;
 
-extern "C" int64_t hi3d_groupnorm_ws_floats(int n_samples) {
-  return (int64_t)n_samples * (GN_MAX_CHUNKS + 1) * GN_GROUPS * 2;     // chunk partials + final (mean, rstd)
-}
-
 static int gn_check(const void* x1, int C1, const void* x2, int C2, int n_samples, int64_t rows_per_sample, const char* who) {
   const int C = C1 + C2;
   if (!x1 || n_samples <= 0 || rows_per_sample <= 0 || C1 <= 0 || (C1 % 8) || (C2 % 8) || (C % GN_GROUPS) || C > 4096 ||
@@ -376,67 +285,28 @@ static int gn_check(const void* x1, int C1, const void* x2, int C2, int n_sample
   return 0;
 }
 
-// (sum, sum of squares) per (sample, group) of the LOCAL rows -> sums[n_samples][32][2] (fp32)
-extern "C" int hi3d_groupnorm_sums(const void* x1, int C1, const void* x2, int C2, int n_samples, int64_t rows_per_sample,
-                                   float* sums, float* ws, void* stream) {
-  if (!x2) C2 = 0;
-  int rc = gn_check(x1, C1, x2, C2, n_samples, rows_per_sample, "hi3d_groupnorm_sums");
-  if (rc) return rc;
-  if (!sums || !ws) { set_error("hi3d_groupnorm_sums: null output / workspace"); return -2; }
-  cudaStream_t st = (cudaStream_t)stream;
-  const int C = C1 + C2, CV = C / 8;
-  const int threads = (512 / CV) * CV;
-  const int RL = threads / CV;
-  const long long min_rows = (long long)RL * GN_UNROLL;     // one unrolled sweep per thread at least
-  long long chunks = (GN_TARGET_CTAS + n_samples - 1) / n_samples;
-  const long long max_by_rows = (rows_per_sample + min_rows - 1) / min_rows;
-  if (chunks > max_by_rows) chunks = max_by_rows;
-  if (chunks > GN_MAX_CHUNKS) chunks = GN_MAX_CHUNKS;
-  if (chunks < 1) chunks = 1;
-  long long rpc = (rows_per_sample + chunks - 1) / chunks;
-  rpc = (rpc + RL - 1) / RL * RL;
-  chunks = (rows_per_sample + rpc - 1) / rpc;
-  gn_stats_kernel<<<dim3((unsigned)chunks, n_samples), threads, 0, st>>>((const __half*)x1, C1, (const __half*)x2, C2,
-                                                                        rows_per_sample, rpc, ws);
-  rc = check_launch("hi3d_groupnorm_sums(stats)");
-  if (rc) return rc;
-  gn_finalize_kernel<<<n_samples, 1024, 0, st>>>(ws, (int)chunks, sums);
-  return check_launch("hi3d_groupnorm_sums(finalize)");
-}
-
-// hi3d_groupnorm_apply_stats routes through the same launcher; its extra arguments travel in these thread-locals
-static thread_local const float* g_apply_stats1 = nullptr;
-static thread_local const float* g_apply_stats2 = nullptr;
-static thread_local int g_apply_unit = 0, g_apply_ips = 1;
-
-// y = [silu]((x - mean) * rstd * gamma + beta) with mean / rstd from `sums` over `count_rows` rows per sample
-// (count_rows = rows_per_sample for a single GPU, the GLOBAL row count when the sums were all-reduced over ranks).
+// The one launcher of gn_apply_kernel.  Statistics come from exactly one source: the unit tables stats1 / stats2 (`unit`
+// channels per entry, `ips` images per sample) when stats1 != NULL, else `sums` [n_samples][32][2].  Either way they cover
+// `count_rows` rows per sample: rows_per_sample on one GPU, the GLOBAL row count when the sums were all-reduced over ranks.
 // Sample n of y starts at row n * y_sample_rows + y_row_off (haloed temporal buffers); 0, 0 -> dense like x.
-extern "C" int hi3d_groupnorm_apply(const void* x1, int C1, const void* x2, int C2, int n_samples, int64_t rows_per_sample,
-                                    const float* sums, int64_t count_rows, const float* gamma, const float* beta, float eps,
-                                    int apply_silu, void* y, int64_t y_sample_rows, int64_t y_row_off, void* stream) {
-  return hi3d_groupnorm_apply_halo(x1, C1, x2, C2, n_samples, rows_per_sample, sums, count_rows, gamma, beta, eps, apply_silu,
-                                   y, y_sample_rows, y_row_off, nullptr, nullptr, 0, stream);
-}
-
-extern "C" int hi3d_groupnorm_apply_halo(const void* x1, int C1, const void* x2, int C2, int n_samples, int64_t rows_per_sample,
-                                         const float* sums, int64_t count_rows, const float* gamma, const float* beta, float eps,
-                                         int apply_silu, void* y, int64_t y_sample_rows, int64_t y_row_off, void* y_prev_rank,
-                                         void* y_next_rank, int64_t frame_rows, void* stream) {
-  // frame_rows > 0 selects the haloed form: a NULL neighbour then means "clip boundary", whose local halo slot is zero-filled
-  if (!x2) C2 = 0;
-  int rc = gn_check(x1, C1, x2, C2, n_samples, rows_per_sample, "hi3d_groupnorm_apply");
+// frame_rows > 0 selects the haloed form: a NULL neighbour then means "clip boundary", whose local halo slot is zero-filled.
+static int gn_apply_launch(const char* who, const void* x1, int C1, const void* x2, int C2, int n_samples,
+                           int64_t rows_per_sample, const float* sums, const float* stats1, const float* stats2, int unit, int ips,
+                           int64_t count_rows, const float* gamma, const float* beta, float eps, int apply_silu, void* y,
+                           int64_t y_sample_rows, int64_t y_row_off, void* y_prev_rank, void* y_next_rank, int64_t frame_rows,
+                           void* stream) {
+  int rc = gn_check(x1, C1, x2, C2, n_samples, rows_per_sample, who);
   if (rc) return rc;
   if ((y_prev_rank || y_next_rank || frame_rows > 0) &&
       (frame_rows <= 0 || rows_per_sample % frame_rows || y_sample_rows != rows_per_sample + 2 * frame_rows ||
        y_row_off != frame_rows || ((uintptr_t)y_prev_rank & 15) || ((uintptr_t)y_next_rank & 15))) {
-    set_error("hi3d_groupnorm_apply_halo: the peer halo stores need y = [n, T_local + 2, frame_rows, C] with y_row_off = "
-              "frame_rows (rows %lld, frame_rows %lld, y_sample_rows %lld, y_row_off %lld)", (long long)rows_per_sample,
-              (long long)frame_rows, (long long)y_sample_rows, (long long)y_row_off);
+    set_error("%s: the peer halo stores need y = [n, T_local + 2, frame_rows, C] with y_row_off = frame_rows (rows %lld, "
+              "frame_rows %lld, y_sample_rows %lld, y_row_off %lld)", who, (long long)rows_per_sample, (long long)frame_rows,
+              (long long)y_sample_rows, (long long)y_row_off);
     return -2;
   }
-  if ((!sums && !g_apply_stats1) || !gamma || !beta || !y || ((uintptr_t)y & 15) || count_rows <= 0) {
-    set_error("hi3d_groupnorm_apply: bad arguments");
+  if ((!sums && !stats1) || !gamma || !beta || !y || ((uintptr_t)y & 15) || count_rows <= 0) {
+    set_error("%s: bad arguments", who);
     return -2;
   }
   if (y_sample_rows <= 0) { y_sample_rows = rows_per_sample; y_row_off = 0; }
@@ -454,23 +324,33 @@ extern "C" int hi3d_groupnorm_apply_halo(const void* x1, int C1, const void* x2,
   long long rows_per_cta = (rows_per_sample + slabs - 1) / slabs;
   rows_per_cta = (rows_per_cta + RL - 1) / RL * RL;
   slabs = (rows_per_sample + rows_per_cta - 1) / rows_per_cta;
-  if (slabs > 2147483647LL) { set_error("hi3d_groupnorm_apply: too many slabs"); return -2; }
+  if (slabs > 2147483647LL) { set_error("%s: too many slabs", who); return -2; }
   if (frame_rows > 0)
     gn_apply_kernel<true><<<dim3((unsigned)slabs, n_samples), threads, 0, st>>>(
         (const __half*)x1, C1, (const __half*)x2, C2, rows_per_sample, rows_per_cta, sums,
         (double)count_rows * (double)(C / GN_GROUPS), eps, gamma, beta, apply_silu, (__half*)y, y_sample_rows, y_row_off,
-        (__half*)y_prev_rank, (__half*)y_next_rank, frame_rows, !y_prev_rank ? 1 : 0, !y_next_rank ? 1 : 0, g_apply_stats1,
-        g_apply_stats2, g_apply_unit, g_apply_ips);
+        (__half*)y_prev_rank, (__half*)y_next_rank, frame_rows, !y_prev_rank ? 1 : 0, !y_next_rank ? 1 : 0, stats1, stats2,
+        unit, ips);
   else
     gn_apply_kernel<false><<<dim3((unsigned)slabs, n_samples), threads, 0, st>>>(
         (const __half*)x1, C1, (const __half*)x2, C2, rows_per_sample, rows_per_cta, sums,
         (double)count_rows * (double)(C / GN_GROUPS), eps, gamma, beta, apply_silu, (__half*)y, y_sample_rows, y_row_off,
-        nullptr, nullptr, 0, 0, 0, g_apply_stats1, g_apply_stats2, g_apply_unit, g_apply_ips);
-  return check_launch("hi3d_groupnorm_apply");
+        nullptr, nullptr, 0, 0, 0, stats1, stats2, unit, ips);
+  return check_launch(who);
+}
+
+extern "C" int hi3d_groupnorm_apply_halo(const void* x1, int C1, const void* x2, int C2, int n_samples, int64_t rows_per_sample,
+                                         const float* sums, int64_t count_rows, const float* gamma, const float* beta, float eps,
+                                         int apply_silu, void* y, int64_t y_sample_rows, int64_t y_row_off, void* y_prev_rank,
+                                         void* y_next_rank, int64_t frame_rows, void* stream) {
+  if (!x2) C2 = 0;
+  return gn_apply_launch("hi3d_groupnorm_apply_halo", x1, C1, x2, C2, n_samples, rows_per_sample, sums, nullptr, nullptr, 0, 1,
+                         count_rows, gamma, beta, eps, apply_silu, y, y_sample_rows, y_row_off, y_prev_rank, y_next_rank,
+                         frame_rows, stream);
 }
 
 // ---- unit statistics of an existing tensor: (sum, sumsq) per image and per `unit` consecutive channels, accumulated -------
-// grid (chunks, n_images); same streaming pattern as gn_stats_kernel, folding into units instead of the 32 groups.
+// grid (chunks, n_images); each thread owns one 16-byte channel column and walks rows, then folds its 8 channels into units.
 constexpr int GN_MAX_UNITS = 256;
 __global__ void __launch_bounds__(512)
 gn_unit_stats_kernel(const __half* __restrict__ x, int C, long long rows_per_image, long long rows_per_chunk, int unit,
@@ -605,22 +485,9 @@ extern "C" int hi3d_groupnorm_apply_stats(const void* x1, int C1, const float* s
   if (!stats1 || (x2 && !stats2) || imgs_per_sample <= 0) { set_error("hi3d_groupnorm_apply_stats: null statistics table"); return -2; }
   int rc = unit_check(C1, C2, unit, "hi3d_groupnorm_apply_stats");
   if (rc) return rc;
-  g_apply_stats1 = stats1; g_apply_stats2 = stats2; g_apply_unit = unit; g_apply_ips = imgs_per_sample;
-  rc = hi3d_groupnorm_apply_halo(x1, C1, x2, C2, n_samples, rows_per_sample, nullptr, count_rows, gamma, beta, eps, apply_silu, y,
-                                 y_sample_rows, y_row_off, y_prev_rank, y_next_rank, frame_rows, stream);
-  g_apply_stats1 = g_apply_stats2 = nullptr; g_apply_unit = 0; g_apply_ips = 1;
-  return rc;
-}
-
-extern "C" int hi3d_groupnorm_silu(const void* x1, int C1, const void* x2, int C2, int n_samples,
-                                   int64_t rows_per_sample, const float* gamma, const float* beta, float eps,
-                                   int apply_silu, void* y, float* ws, void* stream) {
-  if (!ws) { set_error("hi3d_groupnorm_silu: null workspace"); return -2; }
-  float* sums = ws + (long long)n_samples * GN_MAX_CHUNKS * GN_GROUPS * 2;
-  int rc = hi3d_groupnorm_sums(x1, C1, x2, C2, n_samples, rows_per_sample, sums, ws, stream);
-  if (rc) return rc;
-  return hi3d_groupnorm_apply(x1, C1, x2, C2, n_samples, rows_per_sample, sums, rows_per_sample, gamma, beta, eps, apply_silu,
-                              y, 0, 0, stream);
+  return gn_apply_launch("hi3d_groupnorm_apply_stats", x1, C1, x2, C2, n_samples, rows_per_sample, nullptr, stats1, stats2, unit,
+                         imgs_per_sample, count_rows, gamma, beta, eps, apply_silu, y, y_sample_rows, y_row_off, y_prev_rank,
+                         y_next_rank, frame_rows, stream);
 }
 
 extern "C" int hi3d_layernorm(const void* x, const void* addvec, int add_div, int add_mod, int64_t M, int C,

@@ -146,32 +146,6 @@ class Gemm:
 
 
 # ------------------------------------------------------------------------------------------------------
-def groupnorm_ws(n_samples: int, device) -> torch.Tensor:
-    return torch.empty(int(N.load().hi3d_groupnorm_ws_floats(n_samples)), dtype=torch.float32, device=device)
-
-
-def groupnorm_silu(x1: torch.Tensor, x2: Optional[torch.Tensor], n_samples: int, rows_per_sample: int,
-                   gamma: torch.Tensor, beta: torch.Tensor, eps: float, silu: bool, y: torch.Tensor,
-                   ws: torch.Tensor):
-    _chk16(x1, "x1"); _chk16(y, "y"); _chk32(gamma, "gamma"); _chk32(beta, "beta")
-    c2 = 0
-    if x2 is not None:
-        _chk16(x2, "x2")
-        c2 = x2.shape[-1]
-    N.check(N.load().hi3d_groupnorm_silu(x1.data_ptr(), x1.shape[-1], _ptr(x2), c2, n_samples, rows_per_sample,
-                                         gamma.data_ptr(), beta.data_ptr(), eps, int(silu), y.data_ptr(),
-                                         ws.data_ptr(), _stream()), "hi3d_groupnorm_silu")
-
-
-def groupnorm_sums(x1: torch.Tensor, x2: Optional[torch.Tensor], n_samples: int, rows_per_sample: int, sums: torch.Tensor,
-                   ws: torch.Tensor):
-    """Local (sum, sumsq) per (sample, group) -> sums fp32 [n_samples, 32, 2] (all-reduced by the caller when sharded)."""
-    _chk16(x1, "x1"); _chk32(sums, "sums")
-    c2 = 0 if x2 is None else x2.shape[-1]
-    N.check(N.load().hi3d_groupnorm_sums(x1.data_ptr(), x1.shape[-1], _ptr(x2), c2, n_samples, rows_per_sample,
-                                         sums.data_ptr(), ws.data_ptr(), _stream()), "hi3d_groupnorm_sums")
-
-
 def groupnorm_apply(x1: torch.Tensor, x2: Optional[torch.Tensor], n_samples: int, rows_per_sample: int, sums: torch.Tensor,
                     count_rows: int, gamma: torch.Tensor, beta: torch.Tensor, eps: float, silu: bool, y: torch.Tensor,
                     y_sample_rows: int = 0, y_row_off: int = 0, y_prev: Optional[int] = None, y_next: Optional[int] = None,
@@ -183,7 +157,7 @@ def groupnorm_apply(x1: torch.Tensor, x2: Optional[torch.Tensor], n_samples: int
     N.check(N.load().hi3d_groupnorm_apply_halo(x1.data_ptr(), x1.shape[-1], _ptr(x2), c2, n_samples, rows_per_sample,
                                                sums.data_ptr(), count_rows, gamma.data_ptr(), beta.data_ptr(), eps, int(silu),
                                                y.data_ptr(), y_sample_rows, y_row_off, y_prev, y_next, frame_rows, _stream()),
-            "hi3d_groupnorm_apply")
+            "hi3d_groupnorm_apply_halo")
 
 
 def groupnorm_apply_stats(x1: torch.Tensor, stats1: torch.Tensor, x2: Optional[torch.Tensor], stats2: Optional[torch.Tensor],

@@ -2,7 +2,7 @@
 
 Same constructor kwargs, same `state_dict` keys/shapes, same `forward` signature and output -- but the
 module is a parameter container plus a *compiled launch plan*: for a given (batch, H, W, T) the whole forward
-is a flat list of C-ABI kernel launches (hi3d_gemm / hi3d_groupnorm_silu / hi3d_layernorm /
+is a flat list of C-ABI kernel launches (hi3d_gemm / hi3d_groupnorm_apply_stats / hi3d_layernorm /
 hi3d_attention_d64 / hi3d_temporal_attention_d64 ...) over pre-allocated channels-last fp16 buffers with
 pre-baked parameter blocks, replayable under a CUDA graph.  There is no per-op nn.Module graph and no
 PyTorch compute on the path.
@@ -316,10 +316,12 @@ class _Plan:
                     self.peer, self.exchange_mode = None, "nccl"
         self.arena = Arena(self.dev, self.peer, ("qkv", "att", "ghalo") if self.peer is not None else ())
         # GroupNorm statistics from the producing GEMM epilogues (hi3d_gemm_params::gn_stats): every GroupNorm is ONE launch
-        # (apply); HI3D_GN_FUSED=0 keeps the separate statistics pass (stats + finalize + apply)
+        # (apply) reading unit tables of model_channels / 32 channels per entry
         self.gn_unit = net.cfg.model_channels // 32
-        self.gn_fused = (os.environ.get("HI3D_GN_FUSED", "1") != "0" and net.cfg.model_channels % 32 == 0
-                         and net.cfg.model_channels * max(net.cfg.channel_mult) // self.gn_unit <= 256)
+        if net.cfg.model_channels % 32 or net.cfg.model_channels * max(net.cfg.channel_mult) // self.gn_unit > 256:
+            raise NotImplementedError(f"GroupNorm statistics tables need model_channels a multiple of 32 and at most 256 units "
+                                      f"per tensor; got model_channels {net.cfg.model_channels}, channel_mult "
+                                      f"{list(net.cfg.channel_mult)}")
         self._stats_floats = 0
         self.stats_arena = None
         self._nvtx_open = False
@@ -343,7 +345,6 @@ class _Plan:
         self.y_h = torch.zeros(N, E, dtype=F16, device=dev)
         self.ctx_in = torch.zeros(N, cfg.context_dim, dtype=F16, device=dev)
         self.ctx_first = torch.zeros(self.B, cfg.context_dim, dtype=F16, device=dev)
-        self.gn_ws = ops.groupnorm_ws(N, dev)
         self.frame_idx = torch.arange(T, dtype=torch.float32, device=dev) + float(self.rank * T)   # global frame ids
         self.gn_sums = torch.zeros(self.B, 32, 2, dtype=torch.float32, device=dev)               # sharded temporal GN
         self.gn_sums_local = torch.zeros(self.B, 32, 2, dtype=torch.float32, device=dev)
@@ -360,7 +361,7 @@ class _Plan:
     # Statistics in the epilogue are free where the main loop hides the epilogue (3x3 convs, wide temporal convs, K >= 1920 --
     # the same threshold as the CTA-pair rule) and cost MORE than a separate statistics pass on the epilogue-bound short-K
     # GEMMs (measured, profiles/r02_gn_epilogue_notes.txt: temporal conv C=320 +165 us per launch against 87 us for the
-    # pass): those keep the pass (hi3d_groupnorm_unit_stats, same table), still one launch less than r01's stats + finalize.
+    # pass): those keep the pass (hi3d_groupnorm_unit_stats, same table).
     GN_FUSE_MIN_K = 1920
 
     def _gemm(self, lst, segs_fn, W, out: LazyBuf, M, gn_defer: bool = False, **kw):
@@ -396,35 +397,26 @@ class _Plan:
                 self._nvtx_open = True
             self._call(self._build, m, kind="marker")
 
-    def _stats(self, n_img: int, C: int) -> Optional[StatsBuf]:
-        if not self.gn_fused:
-            return None
+    def _stats(self, n_img: int, C: int) -> StatsBuf:
         sb = StatsBuf(self, self._stats_floats, n_img, C // self.gn_unit)
         self._stats_floats += n_img * (C // self.gn_unit) * 2
         return sb
 
-    def _gnkw(self, stats: Optional[StatsBuf], rows_per_img: int) -> dict:
+    def _gnkw(self, stats: StatsBuf, rows_per_img: int) -> dict:
         """Gemm kwargs that make its epilogue accumulate the GroupNorm statistics of its output into `stats`."""
-        return {} if stats is None else dict(gn_stats=stats, gn_unit=self.gn_unit, gn_rows=rows_per_img)
+        return dict(gn_stats=stats, gn_unit=self.gn_unit, gn_rows=rows_per_img)
 
-    def _gn(self, lst, srcs, n_samples: int, rows_per_sample: int, ips: int, gb, eps: float, silu: bool, y: LazyBuf,
-            count_rows: Optional[int] = None, **halo):
-        """GroupNorm(32)[+SiLU] of the channel concat of srcs = [(LazyBuf, C, StatsBuf | None), ...] into y.
-        Fused statistics: one apply launch reading the producers' unit tables; otherwise stats + finalize + apply."""
+    def _gn(self, lst, srcs, n_samples: int, rows_per_sample: int, ips: int, gb, eps: float, silu: bool, y: LazyBuf):
+        """GroupNorm(32)[+SiLU] of the channel concat of srcs = [(LazyBuf, C, StatsBuf), ...] into y: one apply launch
+        reading the producers' unit tables."""
         gam, bet = gb
         x1, c1, st1 = srcs[0]
         x2, c2, st2 = srcs[1] if len(srcs) > 1 else (None, 0, None)
         C = c1 + c2
         M = n_samples * rows_per_sample
-        ws = self.gn_ws
-        if self.gn_fused and st1 is not None and (x2 is None or st2 is not None):
-            self._call(lst, lambda: ops.groupnorm_apply_stats(
-                x1.t, st1.t, x2.t if x2 else None, st2.t if x2 else None, self.gn_unit, n_samples, rows_per_sample, ips,
-                count_rows or rows_per_sample, gam, bet, eps, silu, y.t, **halo), kind="groupnorm", bytes=4.0 * M * C)
-        else:
-            assert not halo and count_rows is None
-            self._call(lst, lambda: ops.groupnorm_silu(x1.t, x2.t if x2 else None, n_samples, rows_per_sample, gam, bet, eps,
-                                                       silu, y.t, ws), kind="groupnorm", bytes=6.0 * M * C)
+        self._call(lst, lambda: ops.groupnorm_apply_stats(
+            x1.t, st1.t, x2.t if x2 else None, st2.t if x2 else None, self.gn_unit, n_samples, rows_per_sample, ips,
+            rows_per_sample, gam, bet, eps, silu, y.t), kind="groupnorm", bytes=4.0 * M * C)
 
     def _call(self, lst, fn, **meta):
         """meta: kind / flops / bytes = algorithmic work of the launch (read by bench.py's breakdown)."""
@@ -455,8 +447,8 @@ class _Plan:
         self._gemm(cl, lambda: [ops.SegSpec(self.y_h)], P["label_emb.2"][0], self.label, N, bias=P["label_emb.2"][1])
 
         # ---------------- main body ----------------
-        if self.gn_fused:      # first launch of every forward: the statistics tables the epilogues accumulate into
-            self._call(bl, lambda: self.stats_arena.zero_(), kind="memset")
+        # first launch of every forward: the statistics tables the epilogues accumulate into
+        self._call(bl, lambda: self.stats_arena.zero_(), kind="memset")
         self.xin = A.want("xin", N * H * W, CIN_PAD)
         hs: List[tuple] = []          # (buffer, C, h, w, stats)
         cur: tuple = None
@@ -520,8 +512,7 @@ class _Plan:
 
         # ---------------- materialise buffers, bake launches ----------------
         A.materialise()
-        if self.gn_fused:
-            self.stats_arena = torch.zeros(max(self._stats_floats, 2), dtype=torch.float32, device=self.dev)
+        self.stats_arena = torch.zeros(max(self._stats_floats, 2), dtype=torch.float32, device=self.dev)
         self.steps = [b() for b in self._build]
         self.cond_steps = [b() for b in self._cond_build]
         self._build = self._cond_build = None
@@ -598,7 +589,6 @@ class _Plan:
         g3, b3 = P[q + "gn1"]
         g4, b4 = P[q + "gn2"]
         emb2 = self._emb_slice(q)
-        ws = self.gn_ws
         if self.shard is None:
             self._gn(bl, [(xs, cout, st_xs)], B, T * HW, T, (g3, b3), 1e-5, True, g_mid)
             geo = dict(Ho=HW, Wo=1, T=T)
@@ -619,18 +609,15 @@ class _Plan:
                 (xs, st_xs, (g3, b3), "conv1", hbuf, dict(rowbias=emb2, rb_div=HW, rb_mod=N, **self._gnkw(st_h2, HW))),
                 (hbuf, st_h2, (g4, b4), "conv2", out, dict(residual=xs, blend_x=xs, alpha=P[n + "alpha"],
                                                            **self._gnkw(out_stats, HW)))):
-            def local_sums(dst_sums, src=src, sst=sst):
-                """this rank's (sum, sumsq) per (clip, group): from the producer's unit table, or a statistics pass"""
-                if sst is not None:
-                    return ops.groupnorm_group_sums(sst.t, cout, None, 0, self.gn_unit, B, T, dst_sums)
-                return ops.groupnorm_sums(src.t, None, B, T * HW, dst_sums, ws)
+            def local_sums(dst_sums, sst=sst):
+                """this rank's (sum, sumsq) per (clip, group), folded from the producer's unit table"""
+                return ops.groupnorm_group_sums(sst.t, cout, None, 0, self.gn_unit, B, T, dst_sums)
             if self.peer is not None:
                 # peer memory: partial sums ride on the exchange kernel (all-reduce in one launch); the halo frames are
                 # stored into the neighbours' buffers by the apply kernel itself; a second exchange orders those stores
                 # before the conv (and, with the first, protects the single ghalo buffer from the next writer)
                 pg = self.peer
-                self._call(bl, lambda ls=local_sums: ls(self.gn_sums_local), kind="groupnorm",
-                           bytes=0.0 if sst is not None else 2.0 * M * cout)
+                self._call(bl, lambda ls=local_sums: ls(self.gn_sums_local), kind="groupnorm", bytes=0.0)
                 self._call(bl, lambda: pg.exchange(self.gn_sums_local, self.gn_sums), kind="exchange")
 
                 def apply(src=src, gg=gg, bb=bb):
@@ -642,8 +629,7 @@ class _Plan:
                 self._call(bl, lambda: pg.exchange(), kind="exchange")
             else:
                 from . import dist as D
-                self._call(bl, lambda ls=local_sums: ls(self.gn_sums), kind="groupnorm",
-                           bytes=0.0 if sst is not None else 2.0 * M * cout)
+                self._call(bl, lambda ls=local_sums: ls(self.gn_sums), kind="groupnorm", bytes=0.0)
                 self._call(bl, lambda: D.allreduce_sum_(self.gn_sums), kind="nccl")
                 self._call(bl, lambda src=src, gg=gg, bb=bb: ops.groupnorm_apply(
                     src.t, None, B, T * HW, self.gn_sums, self.Tg * HW, gg, bb, 1e-5, True, gh.t, (T + 2) * HW, HW),
@@ -669,7 +655,6 @@ class _Plan:
         dev = self.dev
         gn, t0, t1, t2 = A.want("gn", M, C), A.want("t0", M, C), A.want("t1", M, C), A.want("t2", M, C)
         ln, qkv, att, ffh = A.want("ln", M, C), A.want("qkv", M, 3 * C), A.want("att", M, C), A.want("ffh", M, 4 * C)
-        ws = self.gn_ws
         # time_pos_embed(timestep_embedding(arange(T))) : plan constant (video_attention.py:266-276)
         tpe_in = torch.zeros(T, C, dtype=F16, device=dev)
         tpe_h = torch.zeros(T, 4 * C, dtype=F16, device=dev)

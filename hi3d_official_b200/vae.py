@@ -36,17 +36,16 @@ class _VAEPlan:
         self.A = Arena(self.dev)
         self._build: List = []
         self.flops = 0.0
-        self.gn_ws = ops.groupnorm_ws(n, self.dev)
         self._pp = 0
         # GroupNorm statistics from the producing GEMM epilogues (hi3d_gemm_params::gn_stats), as in the UNet plan
-        self.gn_unit = max(1, ae.cfg.ch // 32)
-        self.gn_fused = (os.environ.get("HI3D_GN_FUSED", "1") != "0" and ae.cfg.ch % 32 == 0
-                         and ae.cfg.ch * max(ae.cfg.ch_mult) // self.gn_unit <= 256)
+        self.gn_unit = ae.cfg.ch // 32
+        if ae.cfg.ch % 32 or ae.cfg.ch * max(ae.cfg.ch_mult) // self.gn_unit > 256:
+            raise NotImplementedError(f"GroupNorm statistics tables need ch a multiple of 32 and at most 256 units per tensor; "
+                                      f"got ch {ae.cfg.ch}, ch_mult {list(ae.cfg.ch_mult)}")
         self._stats_floats = 0
         self.stats_arena = None
         self._last_stats = {}          # id(LazyBuf) -> StatsBuf of the tensor it currently holds
-        if self.gn_fused:
-            self._call(lambda: self.stats_arena.zero_())
+        self._call(lambda: self.stats_arena.zero_())
         if which == "enc":
             self._compile_encoder()
         elif which == "vdec":
@@ -54,8 +53,7 @@ class _VAEPlan:
         else:
             self._compile_decoder()
         self.A.materialise()
-        if self.gn_fused:
-            self.stats_arena = torch.zeros(max(self._stats_floats, 2), dtype=torch.float32, device=self.dev)
+        self.stats_arena = torch.zeros(max(self._stats_floats, 2), dtype=torch.float32, device=self.dev)
         self.steps = [b() for b in self._build]
         self._build = None
 
@@ -75,7 +73,7 @@ class _VAEPlan:
 
     def _track(self, out: LazyBuf, C: int, rows_per_img: int) -> dict:
         """Gemm kwargs: the epilogue accumulates the GroupNorm statistics of `out` (consumed by the next _gn on it)."""
-        if not self.gn_fused or C % 32 or C % self.gn_unit or C // self.gn_unit > 256:      # (C % 32: never a GroupNorm input)
+        if C % 32 or C % self.gn_unit or C // self.gn_unit > 256:      # (C % 32: never a GroupNorm input)
             self._last_stats.pop((out.tag, out.rows, out.cols), None)
             return {}
         sb = StatsBuf(self, self._stats_floats, self.n, C // self.gn_unit)
@@ -91,12 +89,11 @@ class _VAEPlan:
         """GroupNorm(32)[+swish]; ips = images per sample (T for the (T,H,W) statistics of a time_stack)."""
         g, b = self.P[key]
         st = self._last_stats.get((x.tag, x.rows, x.cols))
+        if st is None:
+            raise RuntimeError(f"VAE plan: no GroupNorm statistics table tracks the input of {key}")
         ns, rows = self.n // ips, rows_per_img * ips
-        if st is not None:
-            self._call(lambda: ops.groupnorm_apply_stats(x.t, st.t, None, None, self.gn_unit, ns, rows, ips, rows, g, b, eps,
-                                                         silu, y.t))
-        else:
-            self._call(lambda: ops.groupnorm_silu(x.t, None, ns, rows, g, b, eps, silu, y.t, self.gn_ws))
+        self._call(lambda: ops.groupnorm_apply_stats(x.t, st.t, None, None, self.gn_unit, ns, rows, ips, rows, g, b, eps, silu,
+                                                     y.t))
 
     def _conv(self, src: LazyBuf, key: str, out: LazyBuf, ho, wo, hs, ws, stride=1, ups=0, pad_lo=1, **kw):
         Wt, b = self.P[key]

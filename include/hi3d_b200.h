@@ -125,49 +125,38 @@ int hi3d_gemm_tc5_set_epilogue_warps(int warps);
 /* ---------------------------------------------------------------------------------------------
  * Normalisation
  * --------------------------------------------------------------------------------------------- */
-/* GroupNorm(32 groups) [+ SiLU] over `rows_per_sample` consecutive rows x (C/32) channels, on the virtual
- * channel-concat of up to two NHWC fp16 sources (x1: C1 channels, x2: C2 channels or NULL).
- * Replaces GroupNorm32 (util.py:274-276; eps 1e-5; temporal ResBlock: rows_per_sample = T*H*W, i.e. the
- * reduction over (C/32, T, H, W) of video_model.py:71-76), Normalize (attention.py:125-128, model.py:52-55;
- * eps 1e-6) and the following nn.SiLU / x*sigmoid(x).  Two launches: partial sums then apply.
- * ws: fp32 workspace of hi3d_groupnorm_ws_floats(n_samples) floats. Output y: fp16 [rows, C1+C2]. */
-int64_t hi3d_groupnorm_ws_floats(int n_samples);
-int hi3d_groupnorm_silu(const void* x1, int C1, const void* x2, int C2, int n_samples, int64_t rows_per_sample,
-                        const float* gamma, const float* beta, float eps, int apply_silu, void* y, float* ws,
-                        void* stream);
+/* GroupNorm(32 groups) [+ SiLU] over `rows_per_sample` consecutive rows x (C/32) channels, on the virtual channel-concat of
+ * up to two NHWC fp16 sources (x1: C1 channels, x2: C2 channels or NULL).  Replaces GroupNorm32 (util.py:274-276; eps 1e-5;
+ * temporal ResBlock: the reduction over (C/32, T, H, W) of video_model.py:71-76), Normalize (attention.py:125-128,
+ * model.py:52-55; eps 1e-6) and the following nn.SiLU / x*sigmoid(x).  Output y: fp16 [rows, C1+C2].
+ *
+ * Statistics travel as unit tables: fp32 [n_images, C/unit, 2] = (sum, sum of squares) per image and per `unit` consecutive
+ * channels, accumulated (zero the table first).  The GEMM that produces a tensor writes its table in the epilogue
+ * (hi3d_gemm_params::gn_stats); hi3d_groupnorm_unit_stats computes the same table from an existing tensor.  unit must divide
+ * C1, C2 and C/32, with at most 256 units per tensor. */
+int hi3d_groupnorm_unit_stats(const void* x, int C, int n_images, int64_t rows_per_image, int unit, float* stats, void* stream);
 
-/* The two halves of hi3d_groupnorm_silu, exposed for frame-sharded runs where the temporal ResBlock's GroupNorm reduces
- * over (C/32, T, H, W) with T split over GPUs (SURVEY F9): `sums` fp32 [n_samples, 32, 2] = (sum, sum of squares) of the
- * local rows; the host all-reduces them over ranks and passes count_rows = the GLOBAL rows per sample.  y may be a
- * haloed buffer: sample n starts at row n * y_sample_rows + y_row_off (0, 0 = dense). */
-int hi3d_groupnorm_sums(const void* x1, int C1, const void* x2, int C2, int n_samples, int64_t rows_per_sample, float* sums,
-                        float* ws, void* stream);
-int hi3d_groupnorm_apply(const void* x1, int C1, const void* x2, int C2, int n_samples, int64_t rows_per_sample,
-                         const float* sums, int64_t count_rows, const float* gamma, const float* beta, float eps,
-                         int apply_silu, void* y, int64_t y_sample_rows, int64_t y_row_off, void* stream);
-
-/* hi3d_groupnorm_apply for frame-sharded runs with the one-frame halo exchange of the temporal (3,1,1) conv fused into its
- * stores: y = [n, T_local + 2, frame_rows, C] (y_sample_rows = (T_local + 2) * frame_rows, y_row_off = frame_rows); the first
- * local frame is also stored into the trailing halo slot of `y_prev_rank` (the same buffer of the rank holding the previous
- * frames, mapped through hi3d_symm_open) and the last local frame into the leading slot of `y_next_rank`; NULL at the clip
- * boundaries: the local halo slot is then zero-filled (the Conv3d zero padding, openaimodel.py:252-261).  A hi3d_peer_exchange must
- * separate this launch from the conv that reads the halo slots. */
-/* The consumer side of hi3d_gemm_params::gn_stats: GroupNorm(32)[+SiLU] whose statistics come from the per-image, per-unit
- * (sum, sumsq) tables written by the GEMM epilogues that produced x1 / x2 (stats1: fp32 [n_images, C1/unit, 2], stats2
- * likewise or NULL) instead of a statistics pass over the tensor: ONE launch per GroupNorm.  Sample n spans images
- * [n*imgs_per_sample, (n+1)*imgs_per_sample) -- 1 for the spatial GroupNorm32, T for the temporal ResBlock's reduction over
- * (C/32, T, H, W) (video_model.py:71-76).  Other arguments as hi3d_groupnorm_apply_halo (frame_rows = 0: dense output). */
+/* GroupNorm(32)[+SiLU] in ONE launch, its statistics read from the unit tables of x1 (stats1) and x2 (stats2, or NULL).
+ * Sample n spans images [n*imgs_per_sample, (n+1)*imgs_per_sample): 1 for the spatial GroupNorm32, T for the temporal
+ * ResBlock.  count_rows = rows per sample the statistics cover (rows_per_sample).  Output layout and halo arguments as
+ * hi3d_groupnorm_apply_halo (y_sample_rows = 0 and frame_rows = 0: dense output like x). */
 int hi3d_groupnorm_apply_stats(const void* x1, int C1, const float* stats1, const void* x2, int C2, const float* stats2,
                                int unit, int n_samples, int64_t rows_per_sample, int imgs_per_sample, int64_t count_rows,
                                const float* gamma, const float* beta, float eps, int apply_silu, void* y, int64_t y_sample_rows,
                                int64_t y_row_off, void* y_prev_rank, void* y_next_rank, int64_t frame_rows, void* stream);
-/* Unit statistics of an existing tensor (same table as hi3d_gemm_params::gn_stats, accumulated): for tensors not produced
- * by an epilogue that can do it (the mma.sync engine uses this internally), and unit tables -> group sums
- * fp32 [n_samples, 32, 2] (what the frame-sharded temporal GroupNorm all-reduces over ranks). */
-int hi3d_groupnorm_unit_stats(const void* x, int C, int n_images, int64_t rows_per_image, int unit, float* stats, void* stream);
+
+/* Frame-sharded runs, where the temporal ResBlock's GroupNorm reduces over (C/32, T, H, W) with T split over GPUs
+ * (SURVEY F9): hi3d_groupnorm_group_sums folds unit tables into `sums` fp32 [n_samples, 32, 2] of the local rows; the host
+ * all-reduces them over ranks and hi3d_groupnorm_apply_halo normalises with count_rows = the GLOBAL rows per sample.
+ * y may be a haloed buffer: sample n starts at row n * y_sample_rows + y_row_off (0, 0 = dense).  With the one-frame halo
+ * exchange of the temporal (3,1,1) conv fused into the stores: y = [n, T_local + 2, frame_rows, C] (y_sample_rows =
+ * (T_local + 2) * frame_rows, y_row_off = frame_rows); the first local frame is also stored into the trailing halo slot of
+ * `y_prev_rank` (the same buffer of the rank holding the previous frames, mapped through hi3d_symm_open) and the last local
+ * frame into the leading slot of `y_next_rank`; NULL at the clip boundaries: the local halo slot is then zero-filled (the
+ * Conv3d zero padding, openaimodel.py:252-261).  A hi3d_peer_exchange must separate this launch from the conv that reads
+ * the halo slots. */
 int hi3d_groupnorm_group_sums(const float* stats1, int C1, const float* stats2, int C2, int unit, int n_samples,
                               int imgs_per_sample, float* sums, void* stream);
-
 int hi3d_groupnorm_apply_halo(const void* x1, int C1, const void* x2, int C2, int n_samples, int64_t rows_per_sample,
                               const float* sums, int64_t count_rows, const float* gamma, const float* beta, float eps,
                               int apply_silu, void* y, int64_t y_sample_rows, int64_t y_row_off, void* y_prev_rank,

@@ -237,8 +237,11 @@ def test_gemm_epilogue_gn_stats_temporal_plain_upconv(pair):
 @pytest.mark.parametrize("silu,eps", [(True, 1e-5), (False, 1e-6)])
 def test_groupnorm_apply_from_unit_stats(silu, eps):
     """hi3d_groupnorm_apply_stats: spatial (per image), temporal (T images per sample) and the two-source concat whose groups
-    straddle the source boundary (C1 = 1280 / 128, C2 = 640 / 64 -> 60 / 6 channels per group), against F.group_norm."""
-    for (n, rows, c1, c2, unit, ips) in ((4, 256, 320, 0, 10, 1), (4, 64, 128, 64, 2, 1), (8, 64, 64, 0, 2, 4), (2, 128, 1280, 640, 10, 1)):
+    straddle the source boundary (C1 = 1280 / 128, C2 = 640 / 64 -> 60 / 6 channels per group), against F.group_norm; also
+    odd row counts (100, 7), a long image (4096 rows) and the 1280 + 1280 skip concat.  unit = gcd(C / 32, C1, C2)."""
+    for (n, rows, c1, c2, unit, ips) in ((4, 256, 320, 0, 10, 1), (4, 64, 128, 64, 2, 1), (8, 64, 64, 0, 2, 4), (2, 128, 1280, 640, 10, 1),
+                                         (3, 100, 320, 0, 10, 1), (4, 64, 192, 128, 2, 1), (2, 16, 1280, 640, 20, 1),
+                                         (2, 4096, 128, 0, 4, 1), (5, 7, 64, 0, 2, 1), (2, 640, 1280, 1280, 80, 1)):
         C = c1 + c2
         x1 = rnd(n * rows, c1, seed=1).to(H) * 1.5 + 0.3
         x2 = (rnd(n * rows, c2, seed=2).to(H) * 0.7 - 0.2) if c2 else None

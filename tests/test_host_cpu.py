@@ -20,7 +20,7 @@ def test_library_exports_every_declared_symbol():
     assert declared == set(_native.EXPORTS), declared ^ set(_native.EXPORTS)
     for s in declared:
         assert hasattr(lib, s)
-    assert lib.hi3d_abi_version() == 2
+    assert lib.hi3d_abi_version() == 3
     # parameter-block layout must match the C struct: 17 ints (+4 pad), 24 segs of 32 bytes, then the tail
     assert _native.GemmParams.seg.offset == 72 and _native.Seg.__dict__["dt"].offset == 28
     import ctypes

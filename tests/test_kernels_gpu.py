@@ -156,24 +156,6 @@ def test_gemm_temporal_conv(T):
 
 
 # ------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("C1,C2,rows,n,silu,eps", [(320, 0, 100, 3, True, 1e-5), (192, 128, 64, 4, True, 1e-5),
-                                                  (1280, 640, 16, 2, False, 1e-6), (128, 0, 4096, 2, True, 1e-6),
-                                                  (64, 0, 7, 5, True, 1e-5), (1280, 1280, 640, 2, True, 1e-5)])
-def test_groupnorm(C1, C2, rows, n, silu, eps):
-    x1 = (rnd(n * rows, C1) * 1.5 + 0.3).to(H)
-    x2 = rnd(n * rows, C2, seed=3).to(H) if C2 else None
-    C = C1 + C2
-    gamma, beta = 1 + 0.1 * rnd(C, seed=4), 0.1 * rnd(C, seed=5)
-    y = torch.zeros(n * rows, C, dtype=H, device=DEV)
-    ws = ops.groupnorm_ws(n, DEV)
-    ops.groupnorm_silu(x1, x2, n, rows, gamma, beta, eps, silu, y, ws)
-    xc = (torch.cat([x1, x2], 1) if C2 else x1).float()
-    ref = F.group_norm(xc.view(n, rows, C).permute(0, 2, 1), 32, gamma, beta, eps)
-    if silu:
-        ref = F.silu(ref)
-    close(y.view(n, rows, C).permute(0, 2, 1), ref, name="groupnorm")
-
-
 @pytest.mark.parametrize("M,C", [(100, 320), (37, 1280), (64, 64), (20, 640), (9, 2560)])
 def test_layernorm(M, C):
     x = (rnd(M, C) * 2 + 0.5).to(H)

@@ -133,7 +133,6 @@ class _GnWorld:
     """x_r [B * Tl * HW, C] per rank, and the haloed GroupNorm outputs gh_r [B * (Tl + 2) * HW, C] (NaN before each apply).
 
     Routes to the statistics, as unet._Plan takes them in peer mode (`_resblock_impl`):
-      "sums"  -- hi3d_groupnorm_sums per rank, summed over ranks in rank order, hi3d_groupnorm_apply_halo;
       "unit"  -- hi3d_groupnorm_unit_stats per rank (the table a producing GEMM epilogue accumulates), then
                  hi3d_groupnorm_group_sums(imgs_per_sample = Tl), summed over ranks, hi3d_groupnorm_apply_halo;
       "stats" -- hi3d_groupnorm_apply_stats with neighbour pointers, reading the ranks' unit tables laid side by side as one
@@ -154,23 +153,19 @@ class _GnWorld:
     def statistics(self, route):
         """What the apply launches read: the all-reduced sums [B, 32, 2], or for route "stats" the gathered unit table.
         (The statistics kernels add with float atomics, so two passes may differ in the last bit: compute them once.)"""
+        assert route in ("unit", "stats"), route
         B, Tl, HW, Cc = self.B, self.Tl, self.HW, self.C
-        if route in ("unit", "stats"):
-            tables = []
-            for x in self.x:
-                t = torch.zeros(B * Tl, Cc // GN_UNIT, 2, device=DEV)
-                ops.groupnorm_unit_stats(x, B * Tl, HW, GN_UNIT, t.view(-1))
-                tables.append(t)
-            if route == "stats":
-                return torch.cat([t.view(B, Tl, -1, 2) for t in tables], 1).contiguous()
+        tables = []
+        for x in self.x:
+            t = torch.zeros(B * Tl, Cc // GN_UNIT, 2, device=DEV)
+            ops.groupnorm_unit_stats(x, B * Tl, HW, GN_UNIT, t.view(-1))
+            tables.append(t)
+        if route == "stats":
+            return torch.cat([t.view(B, Tl, -1, 2) for t in tables], 1).contiguous()
         local = []
-        ws = ops.groupnorm_ws(B, DEV)
         for r in range(self.world):
             s = torch.zeros(B, 32, 2, device=DEV)
-            if route == "sums":
-                ops.groupnorm_sums(self.x[r], None, B, Tl * HW, s, ws)
-            else:
-                ops.groupnorm_group_sums(tables[r].view(-1), Cc, None, 0, GN_UNIT, B, Tl, s)
+            ops.groupnorm_group_sums(tables[r].view(-1), Cc, None, 0, GN_UNIT, B, Tl, s)
             local.append(s)
         total = torch.zeros(B, 32, 2, device=DEV)
         for s in local:                                       # the exchange kernel's all-reduce: rank order
@@ -235,7 +230,7 @@ GN_CASES = [
 ]
 
 
-@pytest.mark.parametrize("route", ["sums", "unit", "stats"])
+@pytest.mark.parametrize("route", ["unit", "stats"])
 @pytest.mark.parametrize("Tl,world,Cc,HW,silu,mean", GN_CASES)
 def test_sharded_temporal_groupnorm_halo(Tl, world, Cc, HW, silu, mean, route):
     gw = _GnWorld(2, Tl, world, Cc, HW, mean=mean, seed=7)
@@ -288,7 +283,7 @@ def test_sharded_temporal_conv_over_halo(pair_mode, engine, pair, path, B, Tl, w
     assert _tc5_tiles(Tl, HW, Cc) == (path == "tc5"), "case id names the wrong engine path"
     pair_mode(pair)
     gw = _GnWorld(B, Tl, world, Cc, HW, seed=11)
-    gw.apply("sums", gw.statistics("sums"), True, range(world))
+    gw.apply("unit", gw.statistics("unit"), True, range(world))
     T, M = Tl * world, B * Tl * HW
     interior = gw.interior()
     _check(interior, gw.reference(True), "conv source interior vs fp32 F.group_norm")
@@ -441,10 +436,10 @@ def test_rejects_groupnorm_halo_geometry():
     rows = Tl * HW
     x = rnd(B * rows, Cc, seed=1).to(H)
     gam, bet = 1 + 0.1 * rnd(Cc, seed=2), 0.1 * rnd(Cc, seed=3)
-    sums = torch.zeros(B, 32, 2, device=DEV)
-    ops.groupnorm_sums(x, None, B, rows, sums, ops.groupnorm_ws(B, DEV))
     table = torch.zeros(B * Tl, Cc // GN_UNIT, 2, device=DEV)
     ops.groupnorm_unit_stats(x, B * Tl, HW, GN_UNIT, table.view(-1))
+    sums = torch.zeros(B, 32, 2, device=DEV)
+    ops.groupnorm_group_sums(table.view(-1), Cc, None, 0, GN_UNIT, B, Tl, sums)
     cap = B * (Tl + 4) * HW               # room for every store the requested geometry could address
     y, yp, yn = _nans(cap, Cc), _nans(cap, Cc), _nans(cap, Cc)
     bad = [((Tl + 3) * HW, HW, HW),       # y_sample_rows != rows + 2 frame_rows
