@@ -117,8 +117,27 @@ class DiffusionEngine(nn.Module):
         return FusedDenoiser(self.denoiser, self.model, shard=shard, **additional_model_inputs)
 
 
+def per_object_randn(shape, generators, device) -> torch.Tensor:
+    """torch.randn(shape) drawn once per object from that object's generator, concatenated along dim 0.  Object i gets
+    exactly the numbers a run that called torch.manual_seed(s_i) draws for the same shape, as long as that run's global
+    generator drew nothing else before; `generators` must live on `device` (CUDA or CPU draws differ)."""
+    return torch.cat([torch.randn(tuple(shape), generator=g, device=device) for g in generators], 0)
+
+
+def randn_like_per_object(parts, generators) -> torch.Tensor:
+    """torch.randn_like(part) for each object's tensor from that object's generator, concatenated along dim 0.  `parts` must be
+    the tensors a single-object run calls randn_like on, views included: randn_like fills memory in the tensor's own stride
+    order, so a permuted view draws the same numbers into different positions than its contiguous copy."""
+    if len(parts) != len(generators):
+        raise ValueError(f"{len(parts)} objects but {len(generators)} generators")
+    return torch.cat([torch.empty_like(p).normal_(generator=g) for p, g in zip(parts, generators)], 0)
+
+
 class VideoLDM(DiffusionEngine):
-    """vtdm/vtdm_gen_v01.py:24-76."""
+    """vtdm/vtdm_gen_v01.py:24-76.
+
+    Batches of objects: every per-frame tensor holds F = B * num_samples frames, object-major (the frames of object 0, then
+    object 1, ...); per-object tensors (crossattn, vector) hold B rows in the same order."""
 
     def __init__(self, num_samples, trained_param_keys=("",), *args, **kwargs):
         self.trained_param_keys = trained_param_keys
@@ -126,8 +145,9 @@ class VideoLDM(DiffusionEngine):
         self.num_samples = num_samples
 
     @torch.no_grad()
-    def add_custom_cond(self, batch, infer=False):
-        """vtdm_gen_v01.py:59-76 (inference branch): cond_aug = 0.02, cond_frames = image + 0.02 * randn."""
+    def add_custom_cond(self, batch, infer=False, generators=None):
+        """vtdm_gen_v01.py:59-76 (inference branch): cond_aug = 0.02, cond_frames = image + 0.02 * randn.
+        batch["video"]: (B, 3, T, H, W).  generators: one CUDA generator per object for the noise (None: the global one)."""
         if not infer:
             raise NotImplementedError("training-time cond_aug sampling is out of scope")
         batch["num_video_frames"] = self.num_samples
@@ -136,7 +156,9 @@ class VideoLDM(DiffusionEngine):
         n = batch["video"].shape[0]
         cond_aug = torch.full((n,), 0.02, device=image.device).half()
         batch["cond_aug"] = cond_aug
-        batch["cond_frames"] = (image + cond_aug.view(-1, 1, 1, 1) * torch.randn_like(image)).half()
+        noise = torch.randn_like(image) if generators is None else \
+            randn_like_per_object([batch["video"][b:b + 1, :, 0] for b in range(n)], generators)
+        batch["cond_frames"] = (image + cond_aug.view(-1, 1, 1, 1) * noise).half()
         if "image_only_indicator" not in batch:
             batch["image_only_indicator"] = torch.zeros((n, self.num_samples), device=image.device).half()
         return batch
@@ -144,7 +166,9 @@ class VideoLDM(DiffusionEngine):
     # ---- hot loop of pipeline_i2v_eval_v01.py:62-98 (after conditioning) ------------------------------------------------------
     @torch.no_grad()
     def sample_stage1(self, c: Dict, uc: Dict, randn: torch.Tensor, decode: bool = True, shard=None):
-        """shard = (rank, world): `randn` and c/uc['concat'] hold only this rank's frames (frame-sharded video); the
+        """randn: (B * T, 4, h, w) for B objects; c / uc: crossattn (B, 1, 1024), vector (B, 768), concat (B * T, 4, h, w).
+        Returns B * T latents or decoded frames, object-major; object i's frames are what a run over object i alone gives.
+        shard = (rank, world): `randn` and c/uc['concat'] hold only this rank's frames (frame-sharded video); the
         returned latents / decoded frames are this rank's frames too."""
         T = self.num_samples
         den = self.bind_denoiser(shard=shard, image_only_indicator=None, num_video_frames=T)
@@ -158,18 +182,24 @@ class VideoLDMStage2(VideoLDM):
     """vtdm/vtdm_gen_stage2_degradeImage.py VideoLDM (inference surface only)."""
 
     @torch.no_grad()
-    def add_custom_cond(self, batch, infer=False):
-        """vtdm_gen_stage2_degradeImage.py:63-86 (inference): cond frames are all T frames of the low-res video."""
+    def add_custom_cond(self, batch, infer=False, generators=None):
+        """vtdm_gen_stage2_degradeImage.py:63-86 (inference): cond frames are all T frames of the low-res video.
+        generators: one CUDA generator per object for the noise (None: the global one)."""
         if not infer:
             raise NotImplementedError("training-time degradation pipeline is out of scope")
         batch["num_video_frames"] = self.num_samples
         video = batch["video"]                                   # (b, c, t, h, w)
-        frames = video.permute(0, 2, 1, 3, 4).reshape(-1, *video.shape[1:2], *video.shape[3:])
+
+        def frames_of(v):                                        # a view for one clip, a copy for several
+            return v.permute(0, 2, 1, 3, 4).reshape(-1, *v.shape[1:2], *v.shape[3:])
+        frames = frames_of(video)
         batch["cond_frames_without_noise"] = video[:, :, 0].half()
         n = video.shape[0]
         cond_aug = torch.full((n,), 0.02, device=video.device).half()
         batch["cond_aug"] = cond_aug
-        batch["cond_frames"] = (frames + 0.02 * torch.randn_like(frames)).half()
+        noise = torch.randn_like(frames) if generators is None else \
+            randn_like_per_object([frames_of(video[b:b + 1]) for b in range(n)], generators)
+        batch["cond_frames"] = (frames + 0.02 * noise).half()
         if "image_only_indicator" not in batch:
             batch["image_only_indicator"] = torch.zeros((n, self.num_samples), device=video.device).half()
         return batch
@@ -178,7 +208,8 @@ class VideoLDMStage2(VideoLDM):
     @torch.no_grad()
     def sample_stage2(self, c: Dict, uc: Dict, init_latents: torch.Tensor, z: torch.Tensor, decode: bool = True,
                       alpha_pow: float = 40.0, shard=None):
-        """init_latents ~ N(0,1) (T,4,h,w) fp32; z = encode_first_stage(low-res frames) (T,4,h,w).
+        """init_latents ~ N(0,1) (B*T,4,h,w) fp32; z = encode_first_stage(low-res frames) (B*T,4,h,w), B objects
+        object-major as in sample_stage1; returns B * T latents or decoded frames.
         shard = (rank, world): all per-frame tensors hold only this rank's frames."""
         from . import ops
         smp = self.sampler

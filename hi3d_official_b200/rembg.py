@@ -21,7 +21,7 @@ MEAN, STD = (0.485, 0.456, 0.406), (0.229, 0.224, 0.225)
 
 
 class U2netSession:
-    """`net`: the network, a callable from a float32 (1, 3, 320, 320) tensor to (1, 320, 320) probabilities."""
+    """`net`: the network, a callable from a float32 (n, 3, 320, 320) tensor to (n, 320, 320) probabilities."""
 
     def __init__(self, net: Callable[[torch.Tensor], torch.Tensor]):
         self.net = net
@@ -36,17 +36,29 @@ class U2netSession:
             tmp[:, :, c] = (im_ary[:, :, c] - MEAN[c]) / STD[c]
         return np.expand_dims(tmp.transpose((2, 0, 1)), 0).astype(np.float32)
 
-    def predict(self, img):
-        """The (img.size) "L" mask of U2netSession.predict."""
-        from PIL import Image
-        x = torch.from_numpy(self.normalize(img))
-        pred = self.net(x)
+    def _run(self, x: np.ndarray) -> np.ndarray:
+        pred = self.net(torch.from_numpy(x))
         pred = pred.detach().float().cpu().numpy() if isinstance(pred, torch.Tensor) else np.asarray(pred, dtype=np.float32)
-        pred = pred.reshape(SIZE[1], SIZE[0])
+        return pred.reshape(x.shape[0], SIZE[1], SIZE[0])
+
+    @staticmethod
+    def _mask(pred: np.ndarray, size):
+        """One image's network output (320, 320) -> its "L" mask at `size`."""
+        from PIL import Image
         ma, mi = np.max(pred), np.min(pred)
         pred = (pred - mi) / (ma - mi)
         mask = Image.fromarray((pred * 255).astype("uint8"), mode="L")
-        return mask.resize(img.size, Image.LANCZOS)
+        return mask.resize(size, Image.LANCZOS)
+
+    def predict(self, img):
+        """The (img.size) "L" mask of U2netSession.predict."""
+        return self._mask(self._run(self.normalize(img))[0], img.size)
+
+    def predict_batch(self, imgs):
+        """predict() for several images of any sizes with ONE network call on (B, 3, 320, 320): rembg's host steps per
+        image, each mask resized back to its own image's size."""
+        pred = self._run(np.concatenate([self.normalize(img) for img in imgs], 0))
+        return [self._mask(p, img.size) for p, img in zip(pred, imgs)]
 
 
 def new_session(state_dict: Optional[Dict[str, torch.Tensor]] = None, device="cuda") -> U2netSession:
@@ -67,3 +79,11 @@ def remove(img, session: U2netSession):
     mask = session.predict(img)
     empty = Image.new("RGBA", img.size, 0)                # naive_cutout
     return Image.composite(img, empty, mask)
+
+
+def remove_batch(imgs, session: U2netSession):
+    """remove() for a list of PIL images of any sizes, with one U^2-Net call over all of them; returns their cut-outs."""
+    from PIL import Image, ImageOps
+    imgs = [ImageOps.exif_transpose(img) for img in imgs]
+    return [Image.composite(img, Image.new("RGBA", img.size, 0), mask)
+            for img, mask in zip(imgs, session.predict_batch(imgs))]

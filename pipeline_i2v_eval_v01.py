@@ -18,6 +18,10 @@ GeneralConditioner, as below.  Otherwise three ways to supply what the towers pr
 Output: <output_dir>/first_step/first.mp4 (8 fps, like v01:96-98,129) + first.pt (the frames as a tensor, which stage 2
 prefers over re-reading the lossy mp4).  Without a checkpoint file the seeded synthetic weights of spec.synth_fill_ are used
 (said loudly).  --tiny builds a reduced-width 2-step model: the smoke size the tests execute this script at.
+
+Several images: --image_path a.png b.png ... writes <output_dir>/<image stem>/{temp_image,first_step}; --elevation, --seed and
+--towers take one value for all or one per image; --batch K samples K objects per batch (background removal, conditioner
+towers, UNet and VAE each run once over the K).  Object i's output is what a run over image i alone with the same seed gives.
 """
 import argparse
 import os
@@ -92,36 +96,51 @@ def remove_background(image_path, output_dir):
     """v01:153-168: rembg.remove with U^2-Net (hi3d_official_b200/rembg.py, weights ckpts/u2net.pth under the working directory),
     the cut-out saved as <output_dir>/temp_image/rgba.png and pasted onto white through its alpha as temp_image/white.png, at
     the input's size.  Returns the image stage 1 reads: white.png, or `image_path` itself when ckpts/u2net.pth is absent."""
+    return remove_backgrounds([image_path], [output_dir])[0]
+
+
+def remove_backgrounds(image_paths, output_dirs):
+    """remove_background for several images with one U^2-Net call (rembg.remove_batch); image i's files go under
+    output_dirs[i]."""
     from PIL import Image
     from hi3d_official_b200 import rembg
     if not os.path.exists(rembg.DEFAULT_WEIGHTS):
-        print(f"[hi3d-b200] WARNING: {rembg.DEFAULT_WEIGHTS} not found, background removal SKIPPED: stage 1 conditions on "
-              f"{image_path} as given, background included", flush=True)
-        return image_path
-    image = rembg.remove(Image.open(image_path), session=rembg.new_session())
-    temp_dir = os.path.join(output_dir, "temp_image")
-    os.makedirs(temp_dir, exist_ok=True)
-    image.save(os.path.join(temp_dir, "rgba.png"))
-    white_path = os.path.join(temp_dir, "white.png")
-    white = Image.new("RGB", image.size, "WHITE")
-    white.paste(image, mask=image.split()[3])
-    white.save(white_path)
-    print(f"[hi3d-b200] removed the background of {image_path}: {white_path}", flush=True)
-    return white_path
+        for image_path in image_paths:
+            print(f"[hi3d-b200] WARNING: {rembg.DEFAULT_WEIGHTS} not found, background removal SKIPPED: stage 1 conditions on "
+                  f"{image_path} as given, background included", flush=True)
+        return list(image_paths)
+    images = rembg.remove_batch([Image.open(p) for p in image_paths], session=rembg.new_session())
+    out = []
+    for image_path, output_dir, image in zip(image_paths, output_dirs, images):
+        temp_dir = os.path.join(output_dir, "temp_image")
+        os.makedirs(temp_dir, exist_ok=True)
+        image.save(os.path.join(temp_dir, "rgba.png"))
+        white_path = os.path.join(temp_dir, "white.png")
+        white = Image.new("RGB", image.size, "WHITE")
+        white.paste(image, mask=image.split()[3])
+        white.save(white_path)
+        print(f"[hi3d-b200] removed the background of {image_path}: {white_path}", flush=True)
+        out.append(white_path)
+    return out
 
 
-def cond_from_towers(model, frames, towers, elevation, stage):
+def cond_from_towers(model, frames, towers, elevation, stage, generators=None):
     """v01:62-78 / v02:104-118: batch -> add_custom_cond -> GeneralConditioner with the third-party towers' outputs supplied.
-    frames: (3, T, H, W) in [-1, 1] on the GPU (stage 1: the image repeated T times)."""
-    T = model.num_samples
-    batch = {"video": frames[None], "elevation": torch.tensor([float(elevation)], device=frames.device),
-             "fps_id": torch.tensor([7.0], device=frames.device), "motion_bucket_id": torch.tensor([127.0], device=frames.device)}
-    batch = model.add_custom_cond(batch, infer=True)
+    frames: (3, T, H, W) for one object or (B, 3, T, H, W) for B, in [-1, 1] on the GPU (stage 1: the image repeated T times).
+    elevation: one number, or one per object.  towers: the objects' tower outputs stacked ('clip' (B, 1024), 'aes' (B, 1),
+    'depth' (B*T, h', w')).  generators: one CUDA generator per object for the condition-frame noise (None: the global one).
+    The conditioner's towers and the VAE encode run once over the whole batch."""
+    video = frames if frames.dim() == 5 else frames[None]
+    B, dev = video.shape[0], frames.device
+    elevs = [float(e) for e in (elevation if isinstance(elevation, (list, tuple)) else [elevation] * B)]
+    batch = {"video": video, "elevation": torch.tensor(elevs, device=dev),
+             "fps_id": torch.full((B,), 7.0, device=dev), "motion_bucket_id": torch.full((B,), 127.0, device=dev)}
+    batch = model.add_custom_cond(batch, infer=True, generators=generators)
     towers = towers or {}                     # a tower missing here runs natively in the conditioner (or raises)
     if "clip" in towers:
-        batch["cond_frames_without_noise:clip"] = towers["clip"].to(frames.device).float().reshape(1, -1)
+        batch["cond_frames_without_noise:clip"] = towers["clip"].to(dev).float().reshape(B, -1)
     if stage == 1 and "aes" in towers:
-        batch["video:aes"] = towers["aes"].to(frames.device).float().reshape(1, 1)
+        batch["video:aes"] = towers["aes"].to(dev).float().reshape(B, 1)
     elif stage == 2 and "depth" in towers:
         batch["cond_frames:depth"] = towers["depth"].to(frames.device).float()
     c, uc = model.conditioner.get_unconditional_conditioning(
@@ -135,20 +154,107 @@ def native_towers_ready(model, allowed_missing=()):
     return missing is not None and not set(missing()) - set(allowed_missing)
 
 
-def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--denoise_config", type=str, default="configs/inference-v01.yaml")
-    ap.add_argument("--denoise_checkpoint", type=str, default="ckpts/first_stage.pt")
-    ap.add_argument("--image_path", type=str, default="demo/15_out.png")
+# ---- several images per run ---------------------------------------------------------------------------------------------
+def add_cli_args(ap, stage):
+    """The flags both entry points share.  --image_path, --elevation, --seed and --towers take one value or one per image."""
+    ap.add_argument("--denoise_config", type=str, default=f"configs/inference-v0{stage}.yaml")
+    ap.add_argument("--denoise_checkpoint", type=str, default="ckpts/first_stage.pt" if stage == 1 else "ckpts/second_stage.pt")
+    ap.add_argument("--image_path", type=str, nargs="+", default=["demo/15_out.png"])
     ap.add_argument("--output_dir", type=str, default="outputs/15_out")
-    ap.add_argument("--elevation", type=int, default=0)
+    ap.add_argument("--elevation", type=int, nargs="+", default=[0])
     ap.add_argument("--cond", type=str, default=None)
-    ap.add_argument("--towers", type=str, default=None)
+    ap.add_argument("--towers", type=str, nargs="+", default=None)
     ap.add_argument("--synthetic", action="store_true")
     ap.add_argument("--tiny", action="store_true")
-    ap.add_argument("--seed", type=int, default=None)
+    ap.add_argument("--seed", type=int, nargs="+", default=None)
+    ap.add_argument("--batch", type=int, default=1,
+                    help="objects per sampling batch (several images): trades device memory for throughput, same results")
+
+
+def per_image(values, n, flag):
+    """One value for all n images, or one per image."""
+    if values is None:
+        return [None] * n
+    if len(values) == 1:
+        return list(values) * n
+    if len(values) != n:
+        raise SystemExit(f"{flag}: give one value or one per image ({n}), got {len(values)}")
+    return list(values)
+
+
+def batch_plan(params):
+    """Several images: per image its output directory <output_dir>/<image stem>, elevation, seed (random when not given)
+    and tower file, and the groups of image indices that share a sampling batch (--batch)."""
+    paths = params.image_path
+    n = len(paths)
+    stems = [os.path.splitext(os.path.basename(p))[0] for p in paths]
+    dup = sorted({s for s in stems if stems.count(s) > 1})
+    if dup:
+        raise SystemExit(f"images with the same file name stem would share an output directory: {dup}")
+    if params.batch < 1:
+        raise SystemExit(f"--batch must be at least 1, got {params.batch}")
+    if params.cond:
+        raise SystemExit("--cond holds one image's conditioning: with several images use --towers, --synthetic or the towers' "
+                         "weights")
+    return dict(dirs=[os.path.join(params.output_dir, s) for s in stems],
+                elevations=per_image(params.elevation, n, "--elevation"),
+                seeds=[random.randint(0, 65535) if s is None else s for s in per_image(params.seed, n, "--seed")],
+                towers=per_image(params.towers, n, "--towers"),
+                groups=[list(range(i, min(n, i + params.batch))) for i in range(0, n, params.batch)])
+
+
+def cat_cond(dicts):
+    """c / uc dictionaries of single objects -> one batch (per-key concatenation, object-major)."""
+    return {k: torch.cat([d[k] for d in dicts], 0) for k in dicts[0]}
+
+
+def load_towers(paths):
+    """--towers files of several images, stacked per key: 'clip' (B, 1024), 'aes' (B, 1), 'depth' (B*T, h', w')."""
+    ts = [torch.load(p) for p in paths]
+    keys = set.intersection(*(set(t) for t in ts))
+    return {k: torch.cat([t[k].float().reshape((-1,) + tuple(t[k].shape[-2:])) if k == "depth" else t[k].float().reshape(1, -1)
+                          for t in ts], 0) for k in keys}
+
+
+def main_batch(params, model, T, h):
+    """Stage 1 over several images, --batch objects per sampling batch; object i draws from its own generators exactly what
+    a single-image run with its seed draws (condition-frame noise, then the initial latents)."""
+    from hi3d_official_b200.engine import per_object_randn
+    plan = batch_plan(params)
+    if not (params.towers or params.synthetic or native_towers_ready(model)):
+        raise SystemExit("the conditioner towers are outside the H100 hot path: pass --towers <file> or --synthetic")
+    for idx in plan["groups"]:
+        seeds, dirs = [plan["seeds"][i] for i in idx], [plan["dirs"][i] for i in idx]
+        gens = [torch.Generator("cuda").manual_seed(s) for s in seeds]
+        if params.synthetic and not params.towers:
+            c, uc = (cat_cond(d) for d in zip(*[synthetic_cond(1, T, h, "cuda", s) for s in seeds]))
+        else:
+            paths = remove_backgrounds([params.image_path[i] for i in idx], dirs)
+            img = torch.stack([load_image(p, 8 * h) for p in paths]).cuda()              # (B, 3, H, W)
+            towers = load_towers([plan["towers"][i] for i in idx]) if params.towers else None
+            c, uc = cond_from_towers(model, img[:, :, None].repeat(1, 1, T, 1, 1), towers,
+                                     [plan["elevations"][i] for i in idx], 1, generators=gens)
+        randn = per_object_randn((T, 4, h, h), gens, "cuda")
+        with torch.no_grad():
+            frames = model.sample_stage1(c, uc, randn)
+        for j, (d, s) in enumerate(zip(dirs, seeds)):
+            mp4 = save_frames(frames[j * T:(j + 1) * T], os.path.join(d, "first_step"), "first")
+            print(f"[hi3d-b200] wrote {T} frames {tuple(frames.shape[1:])} to {mp4} (seed {s})")
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    add_cli_args(ap, 1)
     params = ap.parse_args()
-    seed = random.randint(0, 65535) if params.seed is None else params.seed      # v01:33-34
+    if len(params.image_path) > 1:
+        batch_plan(params)                                                       # argument errors before the model loads
+        model = load_model(params.denoise_config, params.denoise_checkpoint, 1, params.tiny)
+        return main_batch(params, model, model.num_samples, 16 if params.tiny else 64)
+    image_path, elevation = params.image_path[0], params.elevation[0]
+    towers = params.towers[0] if params.towers else None
+    if len(params.elevation) > 1 or (params.seed and len(params.seed) > 1) or (params.towers and len(params.towers) > 1):
+        raise SystemExit("one image takes one --elevation, --seed and --towers value")
+    seed = random.randint(0, 65535) if params.seed is None else params.seed[0]   # v01:33-34
     torch.manual_seed(seed)
     model = load_model(params.denoise_config, params.denoise_checkpoint, 1, params.tiny)
     T = model.num_samples                                                        # 16 frames
@@ -156,14 +262,14 @@ def main():
     if params.cond:
         d = torch.load(params.cond, map_location="cuda")
         c, uc = d["c"], d["uc"]
-    elif params.towers:
-        img = load_image(remove_background(params.image_path, params.output_dir), 8 * h).cuda()
-        c, uc = cond_from_towers(model, img[:, None].repeat(1, T, 1, 1), torch.load(params.towers), params.elevation, 1)
+    elif towers:
+        img = load_image(remove_background(image_path, params.output_dir), 8 * h).cuda()
+        c, uc = cond_from_towers(model, img[:, None].repeat(1, T, 1, 1), torch.load(towers), elevation, 1)
     elif params.synthetic:
         c, uc = synthetic_cond(1, T, h, "cuda", seed)
     elif native_towers_ready(model):
-        img = load_image(remove_background(params.image_path, params.output_dir), 8 * h).cuda()
-        c, uc = cond_from_towers(model, img[:, None].repeat(1, T, 1, 1), None, params.elevation, 1)
+        img = load_image(remove_background(image_path, params.output_dir), 8 * h).cuda()
+        c, uc = cond_from_towers(model, img[:, None].repeat(1, T, 1, 1), None, elevation, 1)
     else:
         raise SystemExit("the conditioner towers are outside the H100 hot path: pass --towers / --cond <file> or --synthetic")
     randn = torch.randn(T, 4, h, h, device="cuda")                               # v01:91
