@@ -9,7 +9,6 @@ namespace hi3d {
 
 constexpr int GN_GROUPS = 32;
 constexpr int GN_UNROLL = 4;
-constexpr int GN_TARGET_CTAS = 132 * 4 * 4;   // ~4 waves at 4 CTAs/SM
 
 HI3D_DEVINL Half8 ld_stream(const __half* p) {
   Half8 v;
@@ -350,87 +349,151 @@ extern "C" int hi3d_groupnorm_apply_halo(const void* x1, int C1, const void* x2,
 }
 
 // ---- unit statistics of an existing tensor: (sum, sumsq) per image and per `unit` consecutive channels, accumulated -------
-// grid (chunks, n_images); each thread owns one 16-byte channel column and walks rows, then folds its 8 channels into units.
+// Every sum is taken in a fixed order that depends on (rows_per_image, C, unit) only, never on scheduling or on the other
+// images of the launch: the same input gives the same table bits, and an image gives the same bits alone or in any batch.
+// Each image is cut into `slices` channel slices (whole units, whole 32-byte sectors) x `ranks` row ranges.  One thread-block
+// cluster of `ranks` CTAs owns one (image, slice):
+//   1. each thread owns one 16-byte channel column of the slice and walks its rows of the CTA's range in order;
+//   2. the CTA folds its row lanes with a fixed pairwise tree in shared memory, then each unit's channels in channel order;
+//   3. after a cluster barrier, rank 0 adds the ranks' unit partials in rank order (distributed shared memory) and adds the
+//      result to the table: one writer per entry per launch, no atomics.
+// The plan (gn_stats_plan) sizes a CTA's share to ~GN_CTA_BYTES, so one large image (the VAE at 1024^2, called one frame at a
+// time) still spreads over up to 8 x slices CTAs, each with GN_STATS_UNROLL 16-byte loads in flight per thread.
 constexpr int GN_MAX_UNITS = 256;
-__global__ void __launch_bounds__(512)
-gn_unit_stats_kernel(const __half* __restrict__ x, int C, long long rows_per_image, long long rows_per_chunk, int unit,
-                     float* __restrict__ stats) {
-  __shared__ float su[GN_MAX_UNITS * 2];
-  const int CV = C >> 3, nu = C / unit;
-  const int tid = threadIdx.x;
-  for (int i = tid; i < nu * 2; i += blockDim.x) su[i] = 0.f;
-  __syncthreads();
-  const int cv = tid % CV, rl = tid / CV, RL = blockDim.x / CV;
-  const int n = blockIdx.y;
-  const long long r0 = (long long)blockIdx.x * rows_per_chunk;
-  long long r1 = r0 + rows_per_chunk;
+constexpr int GN_STATS_THREADS = 512;
+constexpr int GN_STATS_UNROLL = 8;
+constexpr int GN_MAX_RANKS = 8;                       // the portable cluster size
+constexpr long long GN_CTA_BYTES = 256 << 10;
+
+HI3D_DEVINL void cluster_sync_all() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\nbarrier.cluster.wait.acquire.aligned;\n" ::: "memory");
+}
+
+HI3D_DEVINL float ld_cluster_f32(const float* p, unsigned rank) {   // p's counterpart in CTA `rank` of this cluster
+  const uint32_t local = (uint32_t)__cvta_generic_to_shared(p);
+  uint32_t remote;
+  float v;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;\n" : "=r"(remote) : "r"(local), "r"(rank));
+  asm volatile("ld.shared::cluster.f32 %0, [%1];\n" : "=f"(v) : "r"(remote) : "memory");
+  return v;
+}
+
+// (2 CTAs per SM: without the minimum ptxas sinks each load to its use and only one load per thread is in flight)
+__global__ void __launch_bounds__(GN_STATS_THREADS, 2)
+gn_unit_stats_kernel(const __half* __restrict__ x, int C, long long rows_per_image, long long rows_per_rank, int slice_c,
+                     int unit, float* __restrict__ stats) {
+  __shared__ __align__(16) float red[GN_STATS_THREADS * 16];    // [row lane][column][sum 8 | sumsq 8]
+  __shared__ float su[GN_MAX_UNITS * 2];                        // this CTA's unit partials of the slice
+  unsigned rank;
+  asm("mov.u32 %0, %%cluster_ctarank;\n" : "=r"(rank));
+  unsigned ranks;
+  asm("mov.u32 %0, %%cluster_nctarank;\n" : "=r"(ranks));
+  const int tid = threadIdx.x, n = blockIdx.y;
+  const int slice = blockIdx.x / ranks;
+  const int CVs = slice_c >> 3, cv = tid % CVs, rl = tid / CVs, RL = blockDim.x / CVs;   // blockDim.x == RL * CVs
+  const long long r0 = (long long)rank * rows_per_rank;
+  long long r1 = r0 + rows_per_rank;
   if (r1 > rows_per_image) r1 = rows_per_image;
-  const int c0 = cv * 8;
-  const __half* base = x + (long long)n * rows_per_image * C + c0;
+  const __half* base = x + (long long)n * rows_per_image * C + slice * slice_c + cv * 8;
   float s[8], q[8];
 #pragma unroll
   for (int e = 0; e < 8; e++) s[e] = q[e] = 0.f;
-  // four independent 16-byte loads in flight per thread (a read-only stream: memory-level parallelism is the whole game)
-  long long r = r0 + rl;
-  for (; r + 3LL * RL < r1; r += 4LL * RL) {
-    Half8 v[4];
-#pragma unroll
-    for (int u = 0; u < 4; u++) v[u] = ld_stream(base + (r + (long long)u * RL) * C);
-#pragma unroll
-    for (int u = 0; u < 4; u++)
-#pragma unroll
-      for (int k = 0; k < 4; k++) {
-        const float2 f = __half22float2(v[u].h[k]);
-        s[2 * k] += f.x; q[2 * k] += f.x * f.x;
-        s[2 * k + 1] += f.y; q[2 * k + 1] += f.y * f.y;
-      }
-  }
-  for (; r < r1; r += RL) {
-    const Half8 v = ld_stream(base + r * C);
+  auto add = [&](const Half8& v) {
 #pragma unroll
     for (int k = 0; k < 4; k++) {
       const float2 f = __half22float2(v.h[k]);
       s[2 * k] += f.x; q[2 * k] += f.x * f.x;
       s[2 * k + 1] += f.y; q[2 * k + 1] += f.y * f.y;
     }
-  }
-  int ucur = c0 / unit;
-  float as = 0.f, aq = 0.f;
+  };
+  long long r = r0 + rl;
+  for (; r + (long long)(GN_STATS_UNROLL - 1) * RL < r1; r += (long long)GN_STATS_UNROLL * RL) {
+    Half8 v[GN_STATS_UNROLL];
 #pragma unroll
-  for (int e = 0; e < 8; e++) {
-    const int ui = (c0 + e) / unit;
-    if (ui != ucur) {
-      atomicAdd(&su[2 * ucur], as); atomicAdd(&su[2 * ucur + 1], aq);
-      as = aq = 0.f; ucur = ui;
-    }
-    as += s[e]; aq += q[e];
+    for (int u = 0; u < GN_STATS_UNROLL; u++) v[u] = ld_stream(base + (r + (long long)u * RL) * C);
+#pragma unroll
+    for (int u = 0; u < GN_STATS_UNROLL; u++) add(v[u]);
   }
-  atomicAdd(&su[2 * ucur], as); atomicAdd(&su[2 * ucur + 1], aq);
+  for (; r < r1; r += RL) add(ld_stream(base + r * C));
+  float4* mine = reinterpret_cast<float4*>(red + tid * 16);     // tid = rl * CVs + cv: row lane rl's block is contiguous
+  mine[0] = make_float4(s[0], s[1], s[2], s[3]);
+  mine[1] = make_float4(s[4], s[5], s[6], s[7]);
+  mine[2] = make_float4(q[0], q[1], q[2], q[3]);
+  mine[3] = make_float4(q[4], q[5], q[6], q[7]);
   __syncthreads();
-  for (int i = tid; i < nu * 2; i += blockDim.x) atomicAdd(&stats[(long long)n * nu * 2 + i], su[i]);
+  // row lanes: a fixed pairwise tree (lane i += lane i + h while more than one lane is left)
+  const int W16 = CVs * 16;
+  for (int m = RL; m > 1;) {
+    const int h = (m + 1) >> 1, items = (m - h) * W16;
+    for (int i = tid; i < items; i += blockDim.x) red[i] += red[i + h * W16];
+    __syncthreads();
+    m = h;
+  }
+  // channels -> units, in channel order
+  const int nus = slice_c / unit;
+  for (int i = tid; i < nus * 2; i += blockDim.x) {      // (a CTA may have fewer threads than 2 x units: C = 2560 has 320)
+    const int u = i >> 1, which = i & 1;
+    float acc = 0.f;
+    for (int k = 0; k < unit; k++) {
+      const int c = u * unit + k;
+      acc += red[(c >> 3) * 16 + which * 8 + (c & 7)];
+    }
+    su[i] = acc;
+  }
+  cluster_sync_all();
+  if (rank == 0) {
+    for (int i = tid; i < nus * 2; i += blockDim.x) {
+      float acc = 0.f;
+      for (unsigned k = 0; k < ranks; k++) acc += ld_cluster_f32(su + i, k);
+      stats[((long long)n * (C / unit) + (long long)slice * nus) * 2 + i] += acc;
+    }
+  }
+  cluster_sync_all();                                   // the other CTAs' shared memory stays alive until rank 0 has read it
 }
 
-// unit tables -> (sum, sumsq) per (sample, group): sums[n][32][2]
-__global__ void __launch_bounds__(256)
+// unit tables -> (sum, sumsq) per (sample, group): sums[n][32][2].  One thread per (group, sum | sumsq), adding its entries
+// image by image and unit by unit, the loop of gn_apply_kernel's prologue.
+__global__ void __launch_bounds__(GN_GROUPS * 2)
 gn_group_sums_kernel(const float* __restrict__ stats1, int C1, const float* __restrict__ stats2, int C2, int unit, int ips,
                      float* __restrict__ sums) {
-  __shared__ float ssum[GN_GROUPS * 2];
   const int tid = threadIdx.x, n = blockIdx.x;
-  if (tid < GN_GROUPS * 2) ssum[tid] = 0.f;
-  __syncthreads();
+  const int g = tid >> 1, which = tid & 1;
   const int cpg = (C1 + C2) / GN_GROUPS, upg = cpg / unit, u1 = C1 / unit, u2 = C2 / unit;
-  const int items = GN_GROUPS * ips * upg;
-  for (int it = tid; it < items; it += blockDim.x) {
-    const int g = it / (ips * upg), rem = it - g * (ips * upg);
-    const int img = rem / upg, uu = rem - img * upg;
-    const int u = g * upg + uu;
+  float acc = 0.f;
+  for (int img = 0; img < ips; img++) {
     const long long im = (long long)n * ips + img;
-    const float* src = (u < u1) ? stats1 + (im * u1 + u) * 2 : stats2 + (im * u2 + (u - u1)) * 2;
-    atomicAdd(&ssum[2 * g], src[0]);
-    atomicAdd(&ssum[2 * g + 1], src[1]);
+    for (int uu = 0; uu < upg; uu++) {
+      const int u = g * upg + uu;
+      acc += (u < u1) ? __ldg(stats1 + (im * u1 + u) * 2 + which) : __ldg(stats2 + (im * u2 + (u - u1)) * 2 + which);
+    }
   }
-  __syncthreads();
-  if (tid < GN_GROUPS * 2) sums[(long long)n * (GN_GROUPS * 2) + tid] = ssum[tid];
+  sums[(long long)n * (GN_GROUPS * 2) + tid] = acc;
+}
+
+// The decomposition of one image for gn_unit_stats_kernel, from (rows_per_image, C, unit) alone.
+struct GnStatsPlan {
+  int slices, ranks, slice_c, threads;
+  long long rows_per_rank;
+};
+
+static GnStatsPlan gn_stats_plan(long long rows, int C, int unit) {
+  GnStatsPlan p;
+  const long long bytes = rows * (long long)C * 2;
+  long long want = (bytes + GN_CTA_BYTES - 1) / GN_CTA_BYTES;
+  p.ranks = 1;
+  while (p.ranks < GN_MAX_RANKS && 2LL * p.ranks <= want && rows >= 64LL * p.ranks) p.ranks *= 2;
+  // channel slices: whole units, the fewest that reach `want` CTAs per image.  A slice is at least 64 bytes of a row (32
+  // channels); 32-byte slices (16 channels) only while an image has fewer than 64 CTAs (on an H100 80GB HBM3 at 700 W, the
+  // VAE's 1024^2 x 256 tensor, one frame per call, streamed at 1.45 TB/s in 32-byte slices and 2.69 TB/s in 64-byte ones)
+  p.slices = 1;
+  for (int s = 2; (long long)p.slices * p.ranks < want && s <= C / 16; s++)
+    if (C % s == 0 && (C / s) % unit == 0 && (C / s) % 16 == 0 && ((C / s) >= 32 || (long long)p.slices * p.ranks < 64))
+      p.slices = s;
+  p.slice_c = C / p.slices;
+  const int CVs = p.slice_c / 8;
+  p.threads = (GN_STATS_THREADS / CVs) * CVs;
+  p.rows_per_rank = (rows + p.ranks - 1) / p.ranks;
+  return p;
 }
 
 static int unit_check(int C1, int C2, int unit, const char* who) {
@@ -446,23 +509,29 @@ static int unit_check(int C1, int C2, int unit, const char* who) {
 
 extern "C" int hi3d_groupnorm_unit_stats(const void* x, int C, int n_images, int64_t rows_per_image, int unit, float* stats,
                                          void* stream) {
-  if (!x || !stats || C <= 0 || (C % 8) || n_images <= 0 || n_images > 65535 || rows_per_image <= 0 || unit <= 0 ||
-      (C % unit) || C / unit > GN_MAX_UNITS || ((uintptr_t)x & 15)) {
+  if (!x || !stats || C <= 0 || (C % 8) || C > 8 * GN_STATS_THREADS || n_images <= 0 || n_images > 65535 ||
+      rows_per_image <= 0 || unit <= 0 || (C % unit) || C / unit > GN_MAX_UNITS || ((uintptr_t)x & 15)) {
     set_error("hi3d_groupnorm_unit_stats: bad arguments (C=%d unit=%d n=%d rows=%lld)", C, unit, n_images, (long long)rows_per_image);
     return -2;
   }
-  const int CV = C / 8;
-  const int threads = (512 / CV) * CV;
-  const int RL = threads / CV;
-  long long chunks = (GN_TARGET_CTAS + n_images - 1) / n_images;
-  const long long max_by_rows = (rows_per_image + RL * GN_UNROLL - 1) / ((long long)RL * GN_UNROLL);
-  if (chunks > max_by_rows) chunks = max_by_rows;
-  if (chunks < 1) chunks = 1;
-  long long rpc = (rows_per_image + chunks - 1) / chunks;
-  rpc = (rpc + RL - 1) / RL * RL;
-  chunks = (rows_per_image + rpc - 1) / rpc;
-  gn_unit_stats_kernel<<<dim3((unsigned)chunks, n_images), threads, 0, (cudaStream_t)stream>>>((const __half*)x, C, rows_per_image,
-                                                                                              rpc, unit, stats);
+  const GnStatsPlan p = gn_stats_plan(rows_per_image, C, unit);
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3((unsigned)(p.slices * p.ranks), (unsigned)n_images);
+  cfg.blockDim = dim3((unsigned)p.threads);
+  cfg.stream = (cudaStream_t)stream;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = (unsigned)p.ranks;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  const cudaError_t e = cudaLaunchKernelEx(&cfg, gn_unit_stats_kernel, (const __half*)x, C, (long long)rows_per_image,
+                                           p.rows_per_rank, p.slice_c, unit, stats);
+  if (e != cudaSuccess) {
+    set_error("hi3d_groupnorm_unit_stats: cluster launch failed: %s", cudaGetErrorString(e));
+    return -1;
+  }
   return check_launch("hi3d_groupnorm_unit_stats");
 }
 
@@ -472,7 +541,7 @@ extern "C" int hi3d_groupnorm_group_sums(const float* stats1, int C1, const floa
   if (!stats1 || !sums || n_samples <= 0 || imgs_per_sample <= 0) { set_error("hi3d_groupnorm_group_sums: bad arguments"); return -2; }
   int rc = unit_check(C1, C2, unit, "hi3d_groupnorm_group_sums");
   if (rc) return rc;
-  gn_group_sums_kernel<<<n_samples, 256, 0, (cudaStream_t)stream>>>(stats1, C1, stats2, C2, unit, imgs_per_sample, sums);
+  gn_group_sums_kernel<<<n_samples, GN_GROUPS * 2, 0, (cudaStream_t)stream>>>(stats1, C1, stats2, C2, unit, imgs_per_sample, sums);
   return check_launch("hi3d_groupnorm_group_sums");
 }
 

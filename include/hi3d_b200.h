@@ -94,11 +94,12 @@ typedef struct {
   float alpha;
   void* out;                /* fp16 [M, out_ld]                                                        */
   int32_t out_ld;
-  /* GroupNorm statistics of the OUTPUT tensor, produced by the epilogue (the "GN-stats half" of the fused
-   * GroupNorm+SiLU+conv of openaimodel.py:257-261,292-305: the consumer of this tensor is a GroupNorm, whose separate
-   * statistics pass -- one full read of the tensor -- disappears).  gn_stats: fp32 [n_images, N / gn_unit, 2], (sum, sum of
-   * squares) of the stored fp16 values per image and per unit of gn_unit consecutive channels, ACCUMULATED with atomics (the
-   * caller zeroes it); image of a row = (row of the Ho x Wo / HW GEMM grid) / gn_rows.  Units, not the 32 groups, because a
+  /* GroupNorm statistics of the OUTPUT tensor, for the GroupNorm that consumes it (openaimodel.py:257-261,292-305): after
+   * the GEMM has stored the tensor, the same call runs hi3d_groupnorm_unit_stats over it (the last of an up-conv's four
+   * parity-class launches does, once the tensor is complete), with that function's ordering guarantees.
+   * gn_stats: fp32 [n_images, N / gn_unit, 2], (sum, sum of squares) of the stored fp16 values per image and per unit of
+   * gn_unit consecutive channels, ACCUMULATED (the caller zeroes it); image of a row = (row of the Ho x Wo / HW GEMM grid) /
+   * gn_rows.  Units, not the 32 groups, because a
    * consumer may normalise the channel concat of two tensors (video_model.py:491) whose groups straddle the boundary;
    * gn_unit divides every channels-per-group value of the network (model_channels / 32).  NULL = off. */
   float* gn_stats;
@@ -131,9 +132,16 @@ int hi3d_gemm_tc5_set_epilogue_warps(int warps);
  * model.py:52-55; eps 1e-6) and the following nn.SiLU / x*sigmoid(x).  Output y: fp16 [rows, C1+C2].
  *
  * Statistics travel as unit tables: fp32 [n_images, C/unit, 2] = (sum, sum of squares) per image and per `unit` consecutive
- * channels, accumulated (zero the table first).  The GEMM that produces a tensor writes its table in the epilogue
- * (hi3d_gemm_params::gn_stats); hi3d_groupnorm_unit_stats computes the same table from an existing tensor.  unit must divide
- * C1, C2 and C/32, with at most 256 units per tensor. */
+ * channels, accumulated (zero the table first).  The GEMM that produces a tensor fills its table (hi3d_gemm_params::gn_stats)
+ * through hi3d_groupnorm_unit_stats, which computes the table of an existing tensor.  unit must divide C1, C2 and C/32, with
+ * at most 256 units per tensor.
+ *
+ * Reproducibility: hi3d_groupnorm_unit_stats and hi3d_groupnorm_group_sums use no float atomics and sum in a fixed order.
+ *  - The same input gives the same table bits on every call.
+ *  - An image's entries depend only on that image's rows, rows_per_image, C and unit, never on the other images of the
+ *    launch: an image alone and the same image inside any batch get the same bits.
+ *  - Each table entry has exactly one writer per launch, which adds this launch's sum to the value already there; launches
+ *    into the same table are ordered by the stream. */
 int hi3d_groupnorm_unit_stats(const void* x, int C, int n_images, int64_t rows_per_image, int unit, float* stats, void* stream);
 
 /* GroupNorm(32)[+SiLU] in ONE launch, its statistics read from the unit tables of x1 (stats1) and x2 (stats2, or NULL).
