@@ -36,8 +36,7 @@ class GemmParams(C.Structure):
                 ("rb_div", C.c_int32), ("rb_mod", C.c_int32), ("rb_ld", C.c_int32), ("act", C.c_int32),
                 ("residual", C.c_void_p), ("res_ld", C.c_int32),
                 ("blend_x", C.c_void_p), ("blend_ld", C.c_int32), ("alpha", C.c_float),
-                ("out", C.c_void_p), ("out_ld", C.c_int32),
-                ("gn_stats", C.c_void_p), ("gn_unit", C.c_int32), ("gn_rows", C.c_int32)]
+                ("out", C.c_void_p), ("out_ld", C.c_int32)]
 
 
 _lib = None
@@ -140,7 +139,7 @@ def load(build_if_missing: bool = True):
         fn = getattr(lib, name)   # AttributeError if the .so does not export a declared symbol
         fn.restype = res
         fn.argtypes = args
-    if lib.hi3d_abi_version() != 3:
+    if lib.hi3d_abi_version() != 4:
         raise Hi3dError("libhi3d_b200.so ABI version mismatch")
     _lib = lib
     return lib

@@ -70,7 +70,7 @@ __global__ void maxpool3x3s2_kernel(const __half* __restrict__ x, int H, int W, 
 }
 
 // y = [relu](GN(x) + addend), addend = a raw tensor, GN_a(a) or nothing.  Group statistics of each image come from the unit
-// tables of hi3d_gemm_params::gn_stats; grid (row slabs, images), each thread owns one 8-channel column.
+// tables of hi3d_groupnorm_unit_stats; grid (row slabs, images), each thread owns one 8-channel column.
 __global__ void __launch_bounds__(256)
 gn_apply_add_kernel(const __half* __restrict__ x, const float* __restrict__ stats, const float* __restrict__ gamma,
                     const float* __restrict__ beta, const __half* __restrict__ a, const float* __restrict__ a_stats,

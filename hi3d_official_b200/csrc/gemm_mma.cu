@@ -349,19 +349,6 @@ int validate_gemm(const hi3d_gemm_params* p, const char* who) {
   return 0;
 }
 
-// hi3d_gemm_params::gn_stats: a separate statistics pass over the stored tensor.  The four parity-class launches of an
-// up-conv fill one tensor: the pass runs after the last one.
-int gemm_gn_stats_pass(const hi3d_gemm_params* p, void* stream) {
-  if (p->gn_unit <= 0 || (p->N % p->gn_unit) || p->gn_rows <= 0 || (p->M % p->gn_rows) || p->act == HI3D_ACT_GEGLU ||
-      p->out_ld != p->N) {
-    set_error("hi3d_gemm: bad gn_stats arguments (unit %d, rows %d, N %d, out_ld %d)", p->gn_unit, p->gn_rows, p->N, p->out_ld);
-    return -2;
-  }
-  if (p->out_up && !(p->out_py == 1 && p->out_px == 1)) return 0;
-  return hi3d_groupnorm_unit_stats(p->out, p->N, p->M / p->gn_rows, (int64_t)p->gn_rows * (p->out_up ? 4 : 1), p->gn_unit,
-                                   p->gn_stats, stream);
-}
-
 }  // namespace hi3d
 
 using namespace hi3d;
@@ -376,16 +363,12 @@ extern "C" int hi3d_gemm(const hi3d_gemm_params* p, void* stream) {
   const bool wide = c128 <= c64;
   switch (p->mode) {
     case HI3D_ROWS_PLAIN:
-      rc = wide ? launch_gemm<HI3D_ROWS_PLAIN, 128>(*p, st) : launch_gemm<HI3D_ROWS_PLAIN, 64>(*p, st);
-      break;
+      return wide ? launch_gemm<HI3D_ROWS_PLAIN, 128>(*p, st) : launch_gemm<HI3D_ROWS_PLAIN, 64>(*p, st);
     case HI3D_ROWS_CONV2D:
-      rc = wide ? launch_gemm<HI3D_ROWS_CONV2D, 128>(*p, st) : launch_gemm<HI3D_ROWS_CONV2D, 64>(*p, st);
-      break;
+      return wide ? launch_gemm<HI3D_ROWS_CONV2D, 128>(*p, st) : launch_gemm<HI3D_ROWS_CONV2D, 64>(*p, st);
     default:
-      rc = wide ? launch_gemm<HI3D_ROWS_TEMPORAL, 128>(*p, st) : launch_gemm<HI3D_ROWS_TEMPORAL, 64>(*p, st);
+      return wide ? launch_gemm<HI3D_ROWS_TEMPORAL, 128>(*p, st) : launch_gemm<HI3D_ROWS_TEMPORAL, 64>(*p, st);
   }
-  if (rc || p->gn_stats == nullptr) return rc;
-  return gemm_gn_stats_pass(p, stream);
 }
 
 extern "C" const char* hi3d_last_error(void) { return hi3d::g_err; }
@@ -395,7 +378,9 @@ extern "C" int64_t hi3d_launch_count(void) { return (int64_t)hi3d::g_launches.lo
 // checks that each declared symbol is exported.
 // 3: GroupNorm statistics are unit tables only; the entry points of the chunked statistics pass, its workspace and the dense
 // apply over pre-reduced sums are removed.
-extern "C" int hi3d_abi_version(void) { return 3; }
+// 4: hi3d_gemm_params loses gn_stats / gn_unit / gn_rows (its tail; every other field keeps its offset).  A GEMM computes no
+// statistics: the caller runs hi3d_groupnorm_unit_stats on its output.
+extern "C" int hi3d_abi_version(void) { return 4; }
 
 extern "C" int hi3d_device_info(int* sm_count, int* cc_major, int* cc_minor, int* max_smem_optin) {
   int dev = 0;

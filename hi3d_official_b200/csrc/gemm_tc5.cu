@@ -26,7 +26,6 @@
 
 namespace hi3d {
 int validate_gemm(const hi3d_gemm_params* p, const char* who);
-int gemm_gn_stats_pass(const hi3d_gemm_params* p, void* stream);
 
 constexpr int T5_BM = 128;
 constexpr int T5_BK = 64;
@@ -408,14 +407,6 @@ extern "C" int hi3d_gemm_tc5(const hi3d_gemm_params* p, void* stream) {
     tp.seg[i].dy = s.dy; tp.seg[i].dx = s.dx; tp.seg[i].dt = s.dt;
   }
   if (!ok || m_tiles <= 0) return hi3d_gemm(p, stream);
-  if (p->gn_stats != nullptr) {
-    const int hw = (p->mode == HI3D_ROWS_PLAIN) ? p->gn_rows : p->Ho * p->Wo;
-    if (p->gn_unit <= 0 || (p->N % p->gn_unit) || p->gn_rows <= 0 || (p->M % p->gn_rows) || p->act == HI3D_ACT_GEGLU ||
-        (p->mode != HI3D_ROWS_PLAIN && p->gn_rows != hw)) {
-      set_error("hi3d_gemm_tc5: bad gn_stats arguments (unit %d, rows %d, N %d, M %d)", p->gn_unit, p->gn_rows, p->N, p->M);
-      return -2;
-    }
-  }
 
   // Tile pairs (NT = 2): two row tiles share each B tile, halving the B bytes per output row; worth it once the main loop
   // dominates (long K) and there are enough tiles to fill the SMs with pairs.  The hooks force either choice.
@@ -480,17 +471,11 @@ extern "C" int hi3d_gemm_tc5(const hi3d_gemm_params* p, void* stream) {
   tp.out = (__half*)p->out; tp.out_ld = p->out_ld;
 
   const int smem = stages * stage_bytes + 16 * T5_MAX_STAGES + 1024;
-  if (ntile == 2) {
-    rc = BN == 64 ? launch_tc5<64, 2>(tp, (int)grid, smem, st) : launch_tc5<128, 2>(tp, (int)grid, smem, st);
-  } else {
-    switch (BN) {
-      case 64: rc = launch_tc5<64, 1>(tp, (int)grid, smem, st); break;
-      case 128: rc = launch_tc5<128, 1>(tp, (int)grid, smem, st); break;
-      case 192: rc = launch_tc5<192, 1>(tp, (int)grid, smem, st); break;
-      default: rc = launch_tc5<256, 1>(tp, (int)grid, smem, st);
-    }
+  if (ntile == 2) return BN == 64 ? launch_tc5<64, 2>(tp, (int)grid, smem, st) : launch_tc5<128, 2>(tp, (int)grid, smem, st);
+  switch (BN) {
+    case 64: return launch_tc5<64, 1>(tp, (int)grid, smem, st);
+    case 128: return launch_tc5<128, 1>(tp, (int)grid, smem, st);
+    case 192: return launch_tc5<192, 1>(tp, (int)grid, smem, st);
+    default: return launch_tc5<256, 1>(tp, (int)grid, smem, st);
   }
-  if (rc || p->gn_stats == nullptr) return rc;
-  // hi3d_gemm_params::gn_stats: a statistics pass over the stored tensor, as on the mma.sync engine
-  return gemm_gn_stats_pass(p, stream);
 }

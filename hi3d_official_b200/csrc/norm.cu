@@ -37,7 +37,7 @@ gn_apply_kernel(const __half* __restrict__ x1, int C1, const __half* __restrict_
   const int C = C1 + C2, CV = C >> 3, cpg = C / GN_GROUPS;
   const int tid = threadIdx.x, n = blockIdx.y;
   if (stats1 != nullptr) {
-    // statistics from the unit tables the producing GEMM epilogues accumulated (hi3d_gemm_params::gn_stats): group g of
+    // statistics from the unit tables hi3d_groupnorm_unit_stats accumulated over the inputs: group g of
     // sample n = units [g cpg / unit, (g+1) cpg / unit) of the channel concat, over the `ips` images of the sample.
     // 64 threads, one per (group, sum | sumsq), each adding its <= ips * upg table entries in registers (independent loads).
     if (tid < GN_GROUPS * 2) {
@@ -357,7 +357,7 @@ extern "C" int hi3d_groupnorm_apply_halo(const void* x1, int C1, const void* x2,
 //   2. the CTA folds its row lanes with a fixed pairwise tree in shared memory, then each unit's channels in channel order;
 //   3. after a cluster barrier, rank 0 adds the ranks' unit partials in rank order (distributed shared memory) and adds the
 //      result to the table: one writer per entry per launch, no atomics.
-// The plan (gn_stats_plan) sizes a CTA's share to ~GN_CTA_BYTES, so one large image (the VAE at 1024^2, called one frame at a
+// The plan (unit_stats_plan) sizes a CTA's share to ~GN_CTA_BYTES, so one large image (the VAE at 1024^2, called one frame at a
 // time) still spreads over up to 8 x slices CTAs, each with GN_STATS_UNROLL 16-byte loads in flight per thread.
 constexpr int GN_MAX_UNITS = 256;
 constexpr int GN_STATS_THREADS = 512;
@@ -476,7 +476,7 @@ struct GnStatsPlan {
   long long rows_per_rank;
 };
 
-static GnStatsPlan gn_stats_plan(long long rows, int C, int unit) {
+static GnStatsPlan unit_stats_plan(long long rows, int C, int unit) {
   GnStatsPlan p;
   const long long bytes = rows * (long long)C * 2;
   long long want = (bytes + GN_CTA_BYTES - 1) / GN_CTA_BYTES;
@@ -514,7 +514,7 @@ extern "C" int hi3d_groupnorm_unit_stats(const void* x, int C, int n_images, int
     set_error("hi3d_groupnorm_unit_stats: bad arguments (C=%d unit=%d n=%d rows=%lld)", C, unit, n_images, (long long)rows_per_image);
     return -2;
   }
-  const GnStatsPlan p = gn_stats_plan(rows_per_image, C, unit);
+  const GnStatsPlan p = unit_stats_plan(rows_per_image, C, unit);
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3((unsigned)(p.slices * p.ranks), (unsigned)n_images);
   cfg.blockDim = dim3((unsigned)p.threads);

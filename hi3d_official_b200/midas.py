@@ -5,7 +5,7 @@ feeds it (16, 3, sH, sW) frames in [-1, 1] and turns the (16, sH, sW) inverse de
 
 Per call, everything channels-last fp16 with fp32 accumulation, every conv / linear one hi3d_gemm_tc5:
 
-  BiT ResNet-50 trunk   hi3d_dpt_stem_rows -> stem GEMM (GroupNorm statistics from the epilogue) -> hi3d_groupnorm_apply_add
+  BiT ResNet-50 trunk   hi3d_dpt_stem_rows -> stem GEMM -> its GroupNorm statistics -> hi3d_groupnorm_apply_add
                         (GN + ReLU) -> hi3d_maxpool3x3s2_same; per bottleneck conv1 / conv2 / conv3 GEMMs (the weights are
                         standardised once at load) with GN + ReLU applies in between, and one hi3d_groupnorm_apply_add for
                         relu(GN3(conv3) + shortcut), the shortcut being x or GN(downsample conv) of the same pass
@@ -234,11 +234,12 @@ class DPTHybridTower:
         stats_iter = iter(stats_all)
 
         def gemm(segs, w, out, M, mode=ops.ROWS_PLAIN, geom=None, gn_rows=0, **kw):
-            st = None
-            if gn_rows:
-                st = next(stats_iter)
-                kw.update(gn_stats=st, gn_unit=w.shape[0] // 32, gn_rows=gn_rows)
+            """gn_rows > 0: also the GroupNorm unit table of `out` (images of gn_rows rows), which is returned."""
             ops.Gemm(segs, w, out, M, mode=mode, geom=geom, engine="tc5", **kw)()
+            if not gn_rows:
+                return None
+            st = next(stats_iter)
+            ops.groupnorm_unit_stats(out, M // gn_rows, gn_rows, w.shape[0] // 32, st)
             return st
 
         def conv3(x, w, h, wd, out, stride=1, pad_lo=1, **kw):

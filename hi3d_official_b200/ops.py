@@ -78,7 +78,7 @@ class Gemm:
                  geom: Optional[dict] = None, bias: Optional[torch.Tensor] = None,
                  rowbias: Optional[torch.Tensor] = None, rb_div: int = 1, rb_mod: int = 1, act: int = ACT_NONE,
                  residual: Optional[torch.Tensor] = None, blend_x: Optional[torch.Tensor] = None, alpha: float = 0.0,
-                 engine: str = "mma", gn_stats: Optional[torch.Tensor] = None, gn_unit: int = 0, gn_rows: int = 0):
+                 engine: str = "mma"):
         if out.is_contiguous():
             _chk16(out, "out")
             out_ld, out_rows = out.shape[-1], out.numel() // out.shape[-1]
@@ -128,13 +128,8 @@ class Gemm:
         p.out, p.out_ld = out.data_ptr(), out_ld
         if out.shape[-1] < n_out or out_rows < M * (4 if p.out_up else 1):
             raise ValueError(f"out too small: {tuple(out.shape)} for M={M} N_out={n_out}")
-        if gn_stats is not None:      # GroupNorm statistics of the output from the epilogue (hi3d_gemm_params::gn_stats)
-            _chk32(gn_stats, "gn_stats")
-            if gn_unit <= 0 or Nn % gn_unit or gn_rows <= 0 or M % gn_rows or gn_stats.numel() < (M // gn_rows) * (Nn // gn_unit) * 2:
-                raise ValueError(f"gn_stats: unit {gn_unit} / rows {gn_rows} do not fit N={Nn}, M={M}, table {tuple(gn_stats.shape)}")
-            p.gn_stats, p.gn_unit, p.gn_rows = gn_stats.data_ptr(), gn_unit, gn_rows
         self.p = p
-        self._keep = (list(segs), W, out, bias, rowbias, residual, blend_x, gn_stats)   # keep storages alive
+        self._keep = (list(segs), W, out, bias, rowbias, residual, blend_x)   # keep storages alive
         self._fn = N.load().hi3d_gemm_tc5 if engine == "tc5" else N.load().hi3d_gemm
         self.flops = 2.0 * M * Nn * K
         self.out = out
@@ -165,7 +160,7 @@ def groupnorm_apply_stats(x1: torch.Tensor, stats1: torch.Tensor, x2: Optional[t
                           gamma: torch.Tensor, beta: torch.Tensor, eps: float, silu: bool, y: torch.Tensor,
                           y_sample_rows: int = 0, y_row_off: int = 0, y_prev: Optional[int] = None, y_next: Optional[int] = None,
                           frame_rows: int = 0):
-    """GroupNorm(32)[+SiLU] in ONE launch: statistics from the unit tables written by the producing GEMM epilogues."""
+    """GroupNorm(32)[+SiLU] in ONE launch: statistics from the unit tables of x1 / x2 (groupnorm_unit_stats)."""
     _chk16(x1, "x1"); _chk16(y, "y"); _chk32(stats1, "stats1"); _chk32(gamma, "gamma"); _chk32(beta, "beta")
     c2 = 0 if x2 is None else x2.shape[-1]
     if x2 is not None:
@@ -357,7 +352,7 @@ def groupnorm_apply_add(x: torch.Tensor, stats: torch.Tensor, gamma: torch.Tenso
                         y: torch.Tensor, add: Optional[torch.Tensor] = None, add_stats: Optional[torch.Tensor] = None,
                         add_gamma: Optional[torch.Tensor] = None, add_beta: Optional[torch.Tensor] = None, relu: bool = False,
                         eps: float = 1e-5, y_sample_rows: int = 0, y_row_off: int = 0):
-    """y = [relu](GroupNorm32(x) + add | GroupNorm32(add) | 0), statistics from the GEMM epilogue tables (hi3d_groupnorm_apply_add).
+    """y = [relu](GroupNorm32(x) + add | GroupNorm32(add) | 0), statistics from unit tables (hi3d_groupnorm_apply_add).
     x / add fp16 [n_images * rows, C]; stats / add_stats fp32 [n_images, C / unit, 2]."""
     _chk16(x, "x"); _chk16(y, "y"); _chk32(stats, "stats"); _chk32(gamma, "gamma"); _chk32(beta, "beta")
     C_ = x.shape[-1]

@@ -2,8 +2,8 @@
 
 Same constructor kwargs, same `state_dict` keys/shapes, same `forward` signature and output -- but the
 module is a parameter container plus a *compiled launch plan*: for a given (batch, H, W, T) the whole forward
-is a flat list of C-ABI kernel launches (hi3d_gemm / hi3d_groupnorm_apply_stats / hi3d_layernorm /
-hi3d_attention_d64 / hi3d_temporal_attention_d64 ...) over pre-allocated channels-last fp16 buffers with
+is a flat list of C-ABI kernel launches (hi3d_gemm / hi3d_groupnorm_unit_stats / hi3d_groupnorm_apply_stats /
+hi3d_layernorm / hi3d_attention_d64 / hi3d_temporal_attention_d64 ...) over pre-allocated channels-last fp16 buffers with
 pre-baked parameter blocks, replayable under a CUDA graph.  There is no per-op nn.Module graph and no
 PyTorch compute on the path.
 
@@ -107,6 +107,32 @@ class StatsBuf:
     @property
     def t(self) -> torch.Tensor:
         return self.plan.stats_arena[self.off:self.off + self.n_img * self.units * 2]
+
+
+# The two GroupNorm steps of a launch plan (UNet and VAE).  A step carries its kind and algorithmic bytes (bench.py's
+# breakdown) and the tables it writes (`stats_out`) or reads (`stats_in`).
+def emit_unit_stats(lst: list, x: LazyBuf, st: Optional[StatsBuf], unit: int):
+    """Statistics step: accumulate the unit table `st` of x (st.n_img images of x.rows / st.n_img rows), right after the
+    launches that complete x.  st None: no GroupNorm reads x, and nothing is emitted."""
+    if st is None:
+        return
+    fn = lambda: ops.groupnorm_unit_stats(x.t, st.n_img, x.rows // st.n_img, unit, st.t)   # noqa: E731
+    fn.kind, fn.bytes, fn.stats_out = "groupnorm", 2.0 * x.rows * x.cols, st
+    lst.append(lambda: fn)
+
+
+def emit_groupnorm(lst: list, srcs, unit: int, n_samples: int, rows_per_sample: int, ips: int, gb, eps: float, silu: bool,
+                   y: LazyBuf):
+    """GroupNorm(32)[+SiLU] of the channel concat of srcs = [(LazyBuf, StatsBuf), ...] (one or two sources) into y: one apply
+    launch reading the sources' unit tables.  ips = images per sample (T for the (T, H, W) statistics of a temporal ResBlock)."""
+    (x1, st1), (x2, st2) = srcs[0], srcs[1] if len(srcs) > 1 else (None, None)
+    gam, bet = gb
+    fn = lambda: ops.groupnorm_apply_stats(  # noqa: E731
+        x1.t, st1.t, x2.t if x2 else None, st2.t if x2 else None, unit, n_samples, rows_per_sample, ips, rows_per_sample, gam,
+        bet, eps, silu, y.t)
+    fn.kind, fn.bytes = "groupnorm", 4.0 * n_samples * rows_per_sample * sum(x.cols for x, _ in srcs)
+    fn.stats_in = tuple(st for _, st in srcs)
+    lst.append(lambda: fn)
 
 
 class VideoUNet(nn.Module):
@@ -315,8 +341,8 @@ class _Plan:
                               file=sys.stderr)
                     self.peer, self.exchange_mode = None, "nccl"
         self.arena = Arena(self.dev, self.peer, ("qkv", "att", "ghalo") if self.peer is not None else ())
-        # GroupNorm statistics from the producing GEMM epilogues (hi3d_gemm_params::gn_stats): every GroupNorm is ONE launch
-        # (apply) reading unit tables of model_channels / 32 channels per entry
+        # every GroupNorm is ONE launch (apply) reading the unit tables (model_channels / 32 channels per entry) that a
+        # statistics step wrote after each of its inputs' producers
         self.gn_unit = net.cfg.model_channels // 32
         if net.cfg.model_channels % 32 or net.cfg.model_channels * max(net.cfg.channel_mult) // self.gn_unit > 256:
             raise NotImplementedError(f"GroupNorm statistics tables need model_channels a multiple of 32 and at most 256 units "
@@ -358,33 +384,16 @@ class _Plan:
             dist.barrier(group=self.peer.pg)
 
     # ---- helpers -----------------------------------------------------------------------------------------------
-    # Statistics in the epilogue are free where the main loop hides the epilogue (3x3 convs, wide temporal convs, K >= 1920 --
-    # the same threshold as the CTA-pair rule) and cost MORE than a separate statistics pass on the epilogue-bound short-K
-    # GEMMs (measured, profiles/r02_gn_epilogue_notes.txt: temporal conv C=320 +165 us per launch against 87 us for the
-    # pass): those keep the pass (hi3d_groupnorm_unit_stats, same table).
-    GN_FUSE_MIN_K = 1920
-
-    def _gemm(self, lst, segs_fn, W, out: LazyBuf, M, gn_defer: bool = False, **kw):
-        """Defer Gemm construction until buffers exist. segs_fn() -> list[SegSpec]; tensor kwargs may be LazyBuf.
-        gn_defer: the caller adds the separate statistics pass itself (several launches fill one tensor)."""
-        post = None
-        if kw.get("gn_stats") is not None and W.shape[1] < self.GN_FUSE_MIN_K:
-            st, unit, rows = kw.pop("gn_stats"), kw.pop("gn_unit"), kw.pop("gn_rows")
-            if not gn_defer:
-                post = lambda: (lambda: ops.groupnorm_unit_stats(out.t, st.n_img, (out.rows // st.n_img), unit, st.t))
-
+    def _gemm(self, lst, segs_fn, W, out: LazyBuf, M, **kw):
+        """Defer Gemm construction until buffers exist. segs_fn() -> list[SegSpec]; tensor kwargs may be LazyBuf."""
         def build():
             k2 = {}
             for k, v in kw.items():
-                k2[k] = v.t if isinstance(v, (LazyBuf, StatsBuf)) else v
+                k2[k] = v.t if isinstance(v, LazyBuf) else v
             g = ops.Gemm(segs_fn(), W, out.t if isinstance(out, LazyBuf) else out, M, engine=self.engine, **k2)
             self.flops += g.flops if lst is self._build else 0.0
             return g
         lst.append(build)
-        if post is not None:
-            fn = post()
-            fn.kind, fn.bytes = "groupnorm", 2.0 * out.rows * out.cols
-            lst.append(lambda fn=fn: fn)
 
     def _mark(self, name: str):
         """HI3D_NVTX=1: an NVTX range per layer of the launch plan (block name as in the state dict), so that ncu / nsys
@@ -402,24 +411,9 @@ class _Plan:
         self._stats_floats += n_img * (C // self.gn_unit) * 2
         return sb
 
-    def _gnkw(self, stats: StatsBuf, rows_per_img: int) -> dict:
-        """Gemm kwargs that make its epilogue accumulate the GroupNorm statistics of its output into `stats`."""
-        return dict(gn_stats=stats, gn_unit=self.gn_unit, gn_rows=rows_per_img)
-
-    def _gn(self, lst, srcs, n_samples: int, rows_per_sample: int, ips: int, gb, eps: float, silu: bool, y: LazyBuf):
-        """GroupNorm(32)[+SiLU] of the channel concat of srcs = [(LazyBuf, C, StatsBuf), ...] into y: one apply launch
-        reading the producers' unit tables."""
-        gam, bet = gb
-        x1, c1, st1 = srcs[0]
-        x2, c2, st2 = srcs[1] if len(srcs) > 1 else (None, 0, None)
-        C = c1 + c2
-        M = n_samples * rows_per_sample
-        self._call(lst, lambda: ops.groupnorm_apply_stats(
-            x1.t, st1.t, x2.t if x2 else None, st2.t if x2 else None, self.gn_unit, n_samples, rows_per_sample, ips,
-            rows_per_sample, gam, bet, eps, silu, y.t), kind="groupnorm", bytes=4.0 * M * C)
-
     def _call(self, lst, fn, **meta):
-        """meta: kind / flops / bytes = algorithmic work of the launch (read by bench.py's breakdown)."""
+        """meta: kind / flops / bytes = algorithmic work of the launch (read by bench.py's breakdown); stats_in = the
+        GroupNorm tables it reads (as emit_groupnorm's steps)."""
         for k, v in meta.items():
             setattr(fn, k, v)
         lst.append(lambda: fn)
@@ -447,7 +441,7 @@ class _Plan:
         self._gemm(cl, lambda: [ops.SegSpec(self.y_h)], P["label_emb.2"][0], self.label, N, bias=P["label_emb.2"][1])
 
         # ---------------- main body ----------------
-        # first launch of every forward: the statistics tables the epilogues accumulate into
+        # first launch of every forward: zero the tables that the statistics steps accumulate into
         self._call(bl, lambda: self.stats_arena.zero_(), kind="memset")
         self.xin = A.want("xin", N * H * W, CIN_PAD)
         hs: List[tuple] = []          # (buffer, C, h, w, stats)
@@ -465,18 +459,21 @@ class _Plan:
             for li, L in enumerate(blk):
                 last = li == len(blk) - 1
                 tag = f"hs{bi}" if last else None
+                st = self._stats(N, L.cout)
                 if L.kind == "conv_in":
-                    out, st = next_out(N * h * w, L.cout, tag), self._stats(N, L.cout)
-                    self._conv(bl, [self.xin], P[L.name], out, h, w, h, w, **self._gnkw(st, h * w))
+                    out = next_out(N * h * w, L.cout, tag)
+                    self._conv(bl, [self.xin], P[L.name], out, h, w, h, w)
+                    emit_unit_stats(bl, out, st, self.gn_unit)
                 elif L.kind == "res":
-                    out, st = next_out(N * h * w, L.cout, tag), self._stats(N, L.cout)
+                    out = next_out(N * h * w, L.cout, tag)
                     self._resblock(L, [cur], out, st, h, w)
                 elif L.kind == "attn":
-                    out, st = next_out(N * h * w, L.cout, tag), self._stats(N, L.cout)
+                    out = next_out(N * h * w, L.cout, tag)
                     self._transformer(L, cur, out, st, h, w)
                 elif L.kind == "down":
-                    out, st = next_out(N * (h // 2) * (w // 2), L.cout, tag), self._stats(N, L.cout)
-                    self._conv(bl, [cur[0]], P[L.name], out, h // 2, w // 2, h, w, stride=2, **self._gnkw(st, (h // 2) * (w // 2)))
+                    out = next_out(N * (h // 2) * (w // 2), L.cout, tag)
+                    self._conv(bl, [cur[0]], P[L.name], out, h // 2, w // 2, h, w, stride=2)
+                    emit_unit_stats(bl, out, st, self.gn_unit)
                     h, w = h // 2, w // 2
                 cur = (out, L.cout, h, w, st)
             hs.append(cur)
@@ -491,22 +488,25 @@ class _Plan:
             skip = hs.pop()
             assert (skip[2], skip[3]) == (h, w)
             srcs = [cur, skip]
-            for L in blk:
+            for li, L in enumerate(blk):
+                # the up-sampling conv reads its input without a GroupNorm: that input gets no table
+                st = None if li + 1 < len(blk) and blk[li + 1].kind == "up" else self._stats(N, L.cout)
                 if L.kind == "res":
-                    out, st = next_out(N * h * w, L.cout), self._stats(N, L.cout)
+                    out = next_out(N * h * w, L.cout)
                     self._resblock(L, srcs, out, st, h, w)
                 elif L.kind == "attn":
-                    out, st = next_out(N * h * w, L.cout), self._stats(N, L.cout)
+                    out = next_out(N * h * w, L.cout)
                     self._transformer(L, cur, out, st, h, w)
                 elif L.kind == "up":
-                    out, st = next_out(N * 4 * h * w, L.cout), self._stats(N, L.cout)
-                    self._upconv(bl, cur[0], P[L.name], out, h, w, **self._gnkw(st, h * w))
+                    out = next_out(N * 4 * h * w, L.cout)
+                    self._upconv(bl, cur[0], P[L.name], out, h, w)
+                    emit_unit_stats(bl, out, st, self.gn_unit)       # after all four parity launches
                     h, w = 2 * h, 2 * w
                 cur = (out, L.cout, h, w, st)
         # out: GN32 -> SiLU -> conv3x3 (video_model.py:436-440,500-501)
         M = N * h * w
         g = A.want("gn", M, cur[1])
-        self._gn(bl, [(cur[0], cur[1], cur[4])], N, h * w, 1, P["out.gn"], 1e-5, True, g)
+        emit_groupnorm(bl, [(cur[0], cur[4])], self.gn_unit, N, h * w, 1, P["out.gn"], 1e-5, True, g)
         self.net_out = A.want("net_out", M, COUT_PAD)
         self._conv(bl, [g], P["out.conv"], self.net_out, h, w, h, w)
 
@@ -521,28 +521,20 @@ class _Plan:
         return self.net.plan_desc.input_blocks if which == "input" else self.net.plan_desc.output_blocks
 
     # ---- layer emitters ----------------------------------------------------------------------------------------
-    def _conv(self, lst, srcs: List[LazyBuf], wb, out: LazyBuf, ho, wo, hs_, ws_, stride=1, ups=0, **kw):
+    def _conv(self, lst, srcs: List[LazyBuf], wb, out: LazyBuf, ho, wo, hs_, ws_, stride=1, ups=0):
         Wt, b = wb
         M = self.N * ho * wo
         self._gemm(lst, lambda: ops.conv_taps([s.t for s in srcs]), Wt, out, M, mode=ops.ROWS_CONV2D,
-                   geom=dict(Ho=ho, Wo=wo, Hs=hs_, Ws=ws_, stride=stride, ups=ups), bias=b, **kw)
+                   geom=dict(Ho=ho, Wo=wo, Hs=hs_, Ws=ws_, stride=stride, ups=ups), bias=b)
 
-    def _upconv(self, lst, src: LazyBuf, wb, out: LazyBuf, h, w, n_img=None, **kw):
+    def _upconv(self, lst, src: LazyBuf, wb, out: LazyBuf, h, w):
         """Upsample (nearest x2) + conv3x3 (openaimodel.py:154-156) as four parity-class 2x2 convs on the source
         grid with pre-summed taps (pack.pack_upconv_parity): no upsampled tensor, 4/9 of the FLOPs."""
         parity, b = wb
-        n_img = self.N if n_img is None else n_img
-        M = n_img * h * w
-        fused = True
+        M = self.N * h * w
         for (py, px), (Wt, shifts) in parity.items():
-            fused = Wt.shape[1] >= self.GN_FUSE_MIN_K
             self._gemm(lst, lambda shifts=shifts: [ops.SegSpec(src.t, dy=sy, dx=sx) for sy, sx in shifts], Wt, out, M,
-                       mode=ops.ROWS_CONV2D, geom=dict(Ho=h, Wo=w, Hs=h, Ws=w, out_up=1, out_py=py, out_px=px), bias=b,
-                       gn_defer=True, **kw)
-        if kw.get("gn_stats") is not None and not fused:       # one statistics pass over the tensor the four launches filled
-            st, unit = kw["gn_stats"], kw["gn_unit"]
-            self._call(lst, lambda: ops.groupnorm_unit_stats(out.t, st.n_img, out.rows // st.n_img, unit, st.t),
-                       kind="groupnorm", bytes=2.0 * out.rows * out.cols)
+                       mode=ops.ROWS_CONV2D, geom=dict(Ho=h, Wo=w, Hs=h, Ws=w, out_up=1, out_py=py, out_px=px), bias=b)
 
     def _emb_slice(self, q):
         off, n = self.P["emb_off"][q]
@@ -556,8 +548,9 @@ class _Plan:
         """VideoResBlock (video_model.py:62-81) = spatial ResBlock (openaimodel.py:328-354) + temporal ResBlock
         (dims=3, kernel (3,1,1), GroupNorm over (C/32, T, H, W)) + AlphaBlender, as 4 GN launches + 4 GEMMs.
         srcs = [(buffer, C, h, w, stats), ...] (two entries = the skip concat); every GEMM whose output feeds a GroupNorm
-        accumulates that GroupNorm's statistics in its epilogue (`out_stats` for the block output)."""
-        P, A, bl, N, T, B = self.P, self.arena, self._build, self.N, self.T, self.B
+        is followed by a statistics step into that GroupNorm's table (`out_stats` for the block output, None when no
+        GroupNorm reads it)."""
+        P, A, bl, N, T, B, unit = self.P, self.arena, self._build, self.N, self.T, self.B, self.gn_unit
         n = L.name
         HW = h * w
         M = N * HW
@@ -571,33 +564,36 @@ class _Plan:
         xs = A.want("xs", M, cout)
         st_h1, st_xs, st_h2 = self._stats(N, cout), self._stats(N, cout), self._stats(N, cout)
         # -- spatial half
-        self._gn(bl, [(s_[0], s_[1], s_[4]) for s_ in srcs], N, HW, 1, P[n + "gn1"], 1e-5, True, g_in)
+        emit_groupnorm(bl, [(s_[0], s_[4]) for s_ in srcs], unit, N, HW, 1, P[n + "gn1"], 1e-5, True, g_in)
         emb1 = self._emb_slice(n)
         self._gemm(bl, lambda: ops.conv_taps([g_in.t]), P[n + "conv1"][0], hbuf, M, mode=ops.ROWS_CONV2D,
-                   geom=dict(Ho=h, Wo=w, Hs=h, Ws=w), bias=P[n + "conv1"][1], rowbias=emb1, rb_div=HW, rb_mod=N,
-                   **self._gnkw(st_h1, HW))
-        self._gn(bl, [(hbuf, cout, st_h1)], N, HW, 1, P[n + "gn2"], 1e-5, True, g_mid)
+                   geom=dict(Ho=h, Wo=w, Hs=h, Ws=w), bias=P[n + "conv1"][1], rowbias=emb1, rb_div=HW, rb_mod=N)
+        emit_unit_stats(bl, hbuf, st_h1, unit)
+        emit_groupnorm(bl, [(hbuf, st_h1)], unit, N, HW, 1, P[n + "gn2"], 1e-5, True, g_mid)
         if cin != cout:
             self._gemm(bl, lambda: ops.conv_taps([g_mid.t]) + [ops.SegSpec(s_[0].t) for s_ in srcs], P[n + "conv2"][0], xs, M,
-                       mode=ops.ROWS_CONV2D, geom=dict(Ho=h, Wo=w, Hs=h, Ws=w), bias=P[n + "conv2"][1], **self._gnkw(st_xs, HW))
+                       mode=ops.ROWS_CONV2D, geom=dict(Ho=h, Wo=w, Hs=h, Ws=w), bias=P[n + "conv2"][1])
         else:
             assert x2 is None
             self._gemm(bl, lambda: ops.conv_taps([g_mid.t]), P[n + "conv2"][0], xs, M, mode=ops.ROWS_CONV2D,
-                       geom=dict(Ho=h, Wo=w, Hs=h, Ws=w), bias=P[n + "conv2"][1], residual=x1, **self._gnkw(st_xs, HW))
+                       geom=dict(Ho=h, Wo=w, Hs=h, Ws=w), bias=P[n + "conv2"][1], residual=x1)
+        emit_unit_stats(bl, xs, st_xs, unit)
         # -- temporal half: statistics over (T, H, W) per clip, 3-tap conv along frames
         q = n + "time_stack."
         g3, b3 = P[q + "gn1"]
         g4, b4 = P[q + "gn2"]
         emb2 = self._emb_slice(q)
         if self.shard is None:
-            self._gn(bl, [(xs, cout, st_xs)], B, T * HW, T, (g3, b3), 1e-5, True, g_mid)
+            emit_groupnorm(bl, [(xs, st_xs)], unit, B, T * HW, T, (g3, b3), 1e-5, True, g_mid)
             geo = dict(Ho=HW, Wo=1, T=T)
             self._gemm(bl, lambda: ops.temporal_taps(g_mid.t), P[q + "conv1"][0], hbuf, M, mode=ops.ROWS_TEMPORAL, geom=geo,
-                       bias=P[q + "conv1"][1], rowbias=emb2, rb_div=HW, rb_mod=N, **self._gnkw(st_h2, HW))
-            self._gn(bl, [(hbuf, cout, st_h2)], B, T * HW, T, (g4, b4), 1e-5, True, g_mid)
+                       bias=P[q + "conv1"][1], rowbias=emb2, rb_div=HW, rb_mod=N)
+            emit_unit_stats(bl, hbuf, st_h2, unit)
+            emit_groupnorm(bl, [(hbuf, st_h2)], unit, B, T * HW, T, (g4, b4), 1e-5, True, g_mid)
             # x_t = xs + conv(...);  out = alpha*xs + (1-alpha)*x_t   (util.py:358-369)
             self._gemm(bl, lambda: ops.temporal_taps(g_mid.t), P[q + "conv2"][0], out, M, mode=ops.ROWS_TEMPORAL, geom=geo,
-                       bias=P[q + "conv2"][1], residual=xs, blend_x=xs, alpha=P[n + "alpha"], **self._gnkw(out_stats, HW))
+                       bias=P[q + "conv2"][1], residual=xs, blend_x=xs, alpha=P[n + "alpha"])
+            emit_unit_stats(bl, out, out_stats, unit)
             return
         # frames sharded over ranks (SURVEY F9 / 8e): the (T,H,W) statistics need the (sum, sumsq) of every rank, the GN
         # output goes into a haloed [B, T+2, HW, C] buffer whose halo frames come from the neighbour ranks, and the 3-tap
@@ -605,19 +601,18 @@ class _Plan:
         gh = A.want("ghalo", B * (T + 2) * HW, cout)
         geo = dict(Ho=HW, Wo=1, T=T, Tin=T + 2, t_off=1)
         r, R = self.rank, self.world
-        for src, sst, (gg, bb), wkey, dst, extra in (
-                (xs, st_xs, (g3, b3), "conv1", hbuf, dict(rowbias=emb2, rb_div=HW, rb_mod=N, **self._gnkw(st_h2, HW))),
-                (hbuf, st_h2, (g4, b4), "conv2", out, dict(residual=xs, blend_x=xs, alpha=P[n + "alpha"],
-                                                           **self._gnkw(out_stats, HW)))):
+        for src, sst, (gg, bb), wkey, dst, dst_st, extra in (
+                (xs, st_xs, (g3, b3), "conv1", hbuf, st_h2, dict(rowbias=emb2, rb_div=HW, rb_mod=N)),
+                (hbuf, st_h2, (g4, b4), "conv2", out, out_stats, dict(residual=xs, blend_x=xs, alpha=P[n + "alpha"]))):
             def local_sums(dst_sums, sst=sst):
                 """this rank's (sum, sumsq) per (clip, group), folded from the producer's unit table"""
-                return ops.groupnorm_group_sums(sst.t, cout, None, 0, self.gn_unit, B, T, dst_sums)
+                return ops.groupnorm_group_sums(sst.t, cout, None, 0, unit, B, T, dst_sums)
             if self.peer is not None:
                 # peer memory: partial sums ride on the exchange kernel (all-reduce in one launch); the halo frames are
                 # stored into the neighbours' buffers by the apply kernel itself; a second exchange orders those stores
                 # before the conv (and, with the first, protects the single ghalo buffer from the next writer)
                 pg = self.peer
-                self._call(bl, lambda ls=local_sums: ls(self.gn_sums_local), kind="groupnorm", bytes=0.0)
+                self._call(bl, lambda ls=local_sums: ls(self.gn_sums_local), kind="groupnorm", bytes=0.0, stats_in=(sst,))
                 self._call(bl, lambda: pg.exchange(self.gn_sums_local, self.gn_sums), kind="exchange")
 
                 def apply(src=src, gg=gg, bb=bb):
@@ -629,7 +624,7 @@ class _Plan:
                 self._call(bl, lambda: pg.exchange(), kind="exchange")
             else:
                 from . import dist as D
-                self._call(bl, lambda ls=local_sums: ls(self.gn_sums), kind="groupnorm", bytes=0.0)
+                self._call(bl, lambda ls=local_sums: ls(self.gn_sums), kind="groupnorm", bytes=0.0, stats_in=(sst,))
                 self._call(bl, lambda: D.allreduce_sum_(self.gn_sums), kind="nccl")
                 self._call(bl, lambda src=src, gg=gg, bb=bb: ops.groupnorm_apply(
                     src.t, None, B, T * HW, self.gn_sums, self.Tg * HW, gg, bb, 1e-5, True, gh.t, (T + 2) * HW, HW),
@@ -637,6 +632,7 @@ class _Plan:
                 self._call(bl, lambda: D.halo_exchange_(gh.t.view(B, T + 2, HW * cout), r, R), kind="nccl")
             self._gemm(bl, lambda: ops.temporal_taps(gh.t), P[q + wkey][0], dst, M, mode=ops.ROWS_TEMPORAL, geom=geo,
                        bias=P[q + wkey][1], **extra)
+            emit_unit_stats(bl, dst, dst_st, unit)
 
     def _transformer(self, L: Layer, xin: tuple, out: LazyBuf, out_stats, h: int, w: int):
         self._mark(L.name + "SpatialVideoTransformer")
@@ -663,7 +659,7 @@ class _Plan:
         ops.Gemm([ops.SegSpec(tpe_in)], P[n + "tpe0"][0], tpe_h, T, bias=P[n + "tpe0"][1], act=ops.ACT_SILU)()
         ops.Gemm([ops.SegSpec(tpe_h)], P[n + "tpe2"][0], emb_t, T, bias=P[n + "tpe2"][1])()
 
-        self._gn(bl, [(x, C, xin[4])], N, HW, 1, P[n + "norm"], 1e-6, False, gn)
+        emit_groupnorm(bl, [(x, xin[4])], self.gn_unit, N, HW, 1, P[n + "norm"], 1e-6, False, gn)
         self._gemm(bl, lambda: [ops.SegSpec(gn.t)], P[n + "proj_in"][0], t0, M, bias=P[n + "proj_in"][1])
         tok = t0
         for d in range(self.net.cfg.transformer_depth):
@@ -729,8 +725,8 @@ class _Plan:
             self._gemm(bl, lambda: [ops.SegSpec(ffh.t)], P[qt + "ff2"][0], t0, M, bias=P[qt + "ff2"][1], residual=t1,
                        blend_x=t2, alpha=P[n + "alpha"])
             tok = t0
-        self._gemm(bl, lambda: [ops.SegSpec(tok.t)], P[n + "proj_out"][0], out, M, bias=P[n + "proj_out"][1], residual=x,
-                   **self._gnkw(out_stats, HW))
+        self._gemm(bl, lambda: [ops.SegSpec(tok.t)], P[n + "proj_out"][0], out, M, bias=P[n + "proj_out"][1], residual=x)
+        emit_unit_stats(bl, out, out_stats, self.gn_unit)
 
     def _ln(self, lst, x: LazyBuf, gb, y: LazyBuf, M, addvec=None, add_div=1, add_mod=1):
         g, b = gb

@@ -19,7 +19,7 @@ import torch.nn as nn
 
 from . import ops, pack
 from .spec import VAEConfig, vae_param_shapes
-from .unet import Arena, LazyBuf, StatsBuf, _ParamTree
+from .unet import Arena, LazyBuf, StatsBuf, _ParamTree, emit_groupnorm, emit_unit_stats
 
 F16 = torch.float16
 CIN_PAD = 64
@@ -37,14 +37,13 @@ class _VAEPlan:
         self._build: List = []
         self.flops = 0.0
         self._pp = 0
-        # GroupNorm statistics from the producing GEMM epilogues (hi3d_gemm_params::gn_stats), as in the UNet plan
+        # GroupNorm statistics as in the UNet plan: a statistics step after the producer of every GroupNorm input
         self.gn_unit = ae.cfg.ch // 32
         if ae.cfg.ch % 32 or ae.cfg.ch * max(ae.cfg.ch_mult) // self.gn_unit > 256:
             raise NotImplementedError(f"GroupNorm statistics tables need ch a multiple of 32 and at most 256 units per tensor; "
                                       f"got ch {ae.cfg.ch}, ch_mult {list(ae.cfg.ch_mult)}")
         self._stats_floats = 0
         self.stats_arena = None
-        self._last_stats = {}          # id(LazyBuf) -> StatsBuf of the tensor it currently holds
         self._call(lambda: self.stats_arena.zero_())
         if which == "enc":
             self._compile_encoder()
@@ -61,7 +60,7 @@ class _VAEPlan:
     def _gemm(self, segs_fn, W, out, M, **kw):
         def build():
             def res(v):
-                return v.t if isinstance(v, (LazyBuf, StatsBuf)) else (v() if callable(v) else v)
+                return v.t if isinstance(v, LazyBuf) else (v() if callable(v) else v)
             k2 = {k: res(v) for k, v in kw.items()}
             g = ops.Gemm(segs_fn(), res(W), res(out), M, engine=self.ae.engine, **k2)
             self.flops += g.flops
@@ -71,61 +70,52 @@ class _VAEPlan:
     def _call(self, fn):
         self._build.append(lambda: fn)
 
-    def _track(self, out: LazyBuf, C: int, rows_per_img: int) -> dict:
-        """Gemm kwargs: the epilogue accumulates the GroupNorm statistics of `out` (consumed by the next _gn on it)."""
-        if C % 32 or C % self.gn_unit or C // self.gn_unit > 256:      # (C % 32: never a GroupNorm input)
-            self._last_stats.pop((out.tag, out.rows, out.cols), None)
-            return {}
-        sb = StatsBuf(self, self._stats_floats, self.n, C // self.gn_unit)
-        self._stats_floats += self.n * (C // self.gn_unit) * 2
-        self._last_stats[(out.tag, out.rows, out.cols)] = sb
-        return dict(gn_stats=sb, gn_unit=self.gn_unit, gn_rows=rows_per_img)
+    def _stats(self, x: LazyBuf) -> StatsBuf:
+        """Statistics step after the launches that wrote x: the unit table the GroupNorm of x reads."""
+        sb = StatsBuf(self, self._stats_floats, self.n, x.cols // self.gn_unit)
+        self._stats_floats += self.n * sb.units * 2
+        emit_unit_stats(self._build, x, sb, self.gn_unit)
+        return sb
 
     def _nxt(self, rows, C):
         self._pp ^= 1
         return self.A.want(f"blk{self._pp}", rows, C)
 
-    def _gn(self, x: LazyBuf, key: str, rows_per_img: int, y: LazyBuf, silu=True, eps=1e-6, ips=1):
-        """GroupNorm(32)[+swish]; ips = images per sample (T for the (T,H,W) statistics of a time_stack)."""
-        g, b = self.P[key]
-        st = self._last_stats.get((x.tag, x.rows, x.cols))
-        if st is None:
-            raise RuntimeError(f"VAE plan: no GroupNorm statistics table tracks the input of {key}")
-        ns, rows = self.n // ips, rows_per_img * ips
-        self._call(lambda: ops.groupnorm_apply_stats(x.t, st.t, None, None, self.gn_unit, ns, rows, ips, rows, g, b, eps, silu,
-                                                     y.t))
+    def _gn(self, x: LazyBuf, st: StatsBuf, key: str, rows_per_img: int, y: LazyBuf, silu=True, eps=1e-6, ips=1):
+        """GroupNorm(32)[+swish] of x with its unit table st; ips = images per sample (T for the (T,H,W) statistics of a
+        time_stack)."""
+        emit_groupnorm(self._build, [(x, st)], self.gn_unit, self.n // ips, rows_per_img * ips, ips, self.P[key], eps, silu, y)
 
-    def _conv(self, src: LazyBuf, key: str, out: LazyBuf, ho, wo, hs, ws, stride=1, ups=0, pad_lo=1, **kw):
+    def _conv(self, src: LazyBuf, key: str, out: LazyBuf, ho, wo, hs, ws, stride=1, ups=0, pad_lo=1):
         Wt, b = self.P[key]
         self._gemm(lambda: ops.conv_taps([src.t], pad_lo=pad_lo), Wt, out, self.n * ho * wo, mode=ops.ROWS_CONV2D,
-                   geom=dict(Ho=ho, Wo=wo, Hs=hs, Ws=ws, stride=stride, ups=ups), bias=b, **self._track(out, out.cols, ho * wo),
-                   **kw)
+                   geom=dict(Ho=ho, Wo=wo, Hs=hs, Ws=ws, stride=stride, ups=ups), bias=b)
 
-    def _resnet(self, pre: str, x: LazyBuf, cin: int, cout: int, h: int, w: int) -> LazyBuf:
-        """ResnetBlock.forward, model.py:131-151 (temb is None)."""
+    def _resnet(self, pre: str, x: LazyBuf, x_st: StatsBuf, cin: int, cout: int, h: int, w: int, stats=True):
+        """ResnetBlock.forward, model.py:131-151 (temb is None).  x_st: the unit table of x.  Returns (output, its table, or
+        None with stats=False when no GroupNorm reads the output)."""
         M = self.n * h * w
         g1, hb, g2 = self.A.want("gn", M, cin), self.A.want("h", M, cout), self.A.want("gn", M, cout)
         out = self._nxt(M, cout)
-        self._gn(x, pre + "norm1", h * w, g1)
+        self._gn(x, x_st, pre + "norm1", h * w, g1)
         self._conv(g1, pre + "conv1", hb, h, w, h, w)
-        self._gn(hb, pre + "norm2", h * w, g2)
+        self._gn(hb, self._stats(hb), pre + "norm2", h * w, g2)
         Wt, b = self.P[pre + "conv2"]
         geo = dict(Ho=h, Wo=w, Hs=h, Ws=w)
         if cin != cout:    # nin_shortcut 1x1 as one more K segment over the raw input
             self._gemm(lambda: ops.conv_taps([g2.t]) + [ops.SegSpec(x.t)], Wt, out, M, mode=ops.ROWS_CONV2D, geom=geo,
-                       bias=b, **self._track(out, cout, h * w))
+                       bias=b)
         else:
-            self._gemm(lambda: ops.conv_taps([g2.t]), Wt, out, M, mode=ops.ROWS_CONV2D, geom=geo, bias=b, residual=x,
-                       **self._track(out, cout, h * w))
-        return out
+            self._gemm(lambda: ops.conv_taps([g2.t]), Wt, out, M, mode=ops.ROWS_CONV2D, geom=geo, bias=b, residual=x)
+        return out, self._stats(out) if stats else None
 
-    def _video_resnet(self, pre: str, x: LazyBuf, cin: int, cout: int, h: int, w: int) -> LazyBuf:
+    def _video_resnet(self, pre: str, x: LazyBuf, x_st: StatsBuf, cin: int, cout: int, h: int, w: int, stats=True):
         """temporal_ae.VideoResBlock.forward (temporal_ae.py:62-81): the spatial ResnetBlock, then the `time_stack`
         ResBlock(dims=3, kernel (3,1,1), no emb; openaimodel.py:328-354) on the (b, c, t, h, w) view -- GroupNorm over
         (C/32, T, H, W), eps 1e-5 -- and x = a * time_stack(x) + (1 - a) * x with a = sigmoid(mix_factor): NOTE the blend
         weighs the TEMPORAL branch (the UNet's AlphaBlender weighs the spatial one).  time_stack(x) = x + h, so
         out = x + a h = (1 - a) x + a (x + h): the engine's blend epilogue with alpha_engine = 1 - a."""
-        xs = self._resnet(pre, x, cin, cout, h, w)
+        xs, xs_st = self._resnet(pre, x, x_st, cin, cout, h, w)
         T, n = self.T, self.n
         B, HW = n // T, h * w
         M = n * HW
@@ -136,17 +126,16 @@ class _VAEPlan:
         geo = dict(Ho=HW, Wo=1, T=T)
         a = self.P[pre + "mix_factor"]
 
-        self._gn(xs, q + "in_layers.0", HW, g, eps=1e-5, ips=T)
+        self._gn(xs, xs_st, q + "in_layers.0", HW, g, eps=1e-5, ips=T)
         W1, b1 = self.P[q + "in_layers.2"]
-        self._gemm(lambda: ops.temporal_taps(g.t), W1, hb, M, mode=ops.ROWS_TEMPORAL, geom=geo, bias=b1,
-                   **self._track(hb, cout, HW))
-        self._gn(hb, q + "out_layers.0", HW, g, eps=1e-5, ips=T)
+        self._gemm(lambda: ops.temporal_taps(g.t), W1, hb, M, mode=ops.ROWS_TEMPORAL, geom=geo, bias=b1)
+        self._gn(hb, self._stats(hb), q + "out_layers.0", HW, g, eps=1e-5, ips=T)
         W2, b2 = self.P[q + "out_layers.3"]
         self._gemm(lambda: ops.temporal_taps(g.t), W2, out, M, mode=ops.ROWS_TEMPORAL, geom=geo, bias=b2, residual=xs,
-                   blend_x=xs, alpha=1.0 - a, **self._track(out, cout, HW))
-        return out
+                   blend_x=xs, alpha=1.0 - a)
+        return out, self._stats(out) if stats else None
 
-    def _attn(self, pre: str, x: LazyBuf, C: int, h: int, w: int) -> LazyBuf:
+    def _attn(self, pre: str, x: LazyBuf, x_st: StatsBuf, C: int, h: int, w: int):
         """AttnBlock.forward, model.py:180-201: one head, d = C, softmax(q k^T * C^-0.5) v per image, as
         scores = GEMM(q, k) -> row softmax -> GEMM(P, v^T) on the same engine as everything else."""
         n, L = self.n, h * w
@@ -156,13 +145,13 @@ class _VAEPlan:
             # flash attention on wgmma: q|k|v as ONE GEMM, fp32 scores / softmax inside the kernel, no L x L buffer
             g, qkv, o = A.want("gn", M, C), A.want("qkv", M, 3 * C), A.want("att", M, C)
             out = self._nxt(M, C)
-            self._gn(x, pre + "norm", L, g, silu=False)
+            self._gn(x, x_st, pre + "norm", L, g, silu=False)
             Wq, bq = self.P[pre + "qkv"]
             self._gemm(lambda: [ops.SegSpec(g.t)], Wq, qkv, M, bias=bq)
             self._call(lambda: ops.attention_d512(qkv.t, n, L, o.t, float(C) ** -0.5))
             Wo, bo = self.P[pre + "proj_out"]
-            self._gemm(lambda: [ops.SegSpec(o.t)], Wo, out, M, bias=bo, residual=x, **self._track(out, C, L))
-            return out
+            self._gemm(lambda: [ops.SegSpec(o.t)], Wo, out, M, bias=bo, residual=x)
+            return out, self._stats(out)
         # small / odd sizes (L not a multiple of 128) and the mma.sync engine: scores through the GEMM engine, one image at a
         # time (an L x L fp16 buffer of SCALED logits -- fine for the tiny test shapes this path still serves)
         if L % 64:
@@ -170,7 +159,7 @@ class _VAEPlan:
         g, q, k, v, o = (A.want(t, M, C) for t in ("gn", "q", "k", "v", "att"))
         S, vt = A.want("scores", L, L), A.want("vt", C, L)
         out = self._nxt(M, C)
-        self._gn(x, pre + "norm", L, g, silu=False)
+        self._gn(x, x_st, pre + "norm", L, g, silu=False)
         for nm, dst in (("q_scaled", q), ("k", k), ("v", v)):
             Wt, b = self.P[pre + nm]
             self._gemm(lambda: [ops.SegSpec(g.t)], Wt, dst, M, bias=b)
@@ -181,8 +170,8 @@ class _VAEPlan:
             self._call(lambda: ops.softmax_rows(S.t, L, L, 1.0))
             self._gemm(lambda: [ops.SegSpec(S.t)], vt, lambda sl=sl: o.t[sl], L)
         Wo, bo = self.P[pre + "proj_out"]
-        self._gemm(lambda: [ops.SegSpec(o.t)], Wo, out, M, bias=bo, residual=x, **self._track(out, C, L))
-        return out
+        self._gemm(lambda: [ops.SegSpec(o.t)], Wo, out, M, bias=bo, residual=x)
+        return out, self._stats(out)
 
     # -- encoder / decoder walks ----------------------------------------------------------------------------------
     def _compile_encoder(self):
@@ -195,23 +184,28 @@ class _VAEPlan:
         h, w = H, W
         cur = self._nxt(n * h * w, cfg.ch)
         self._conv(self.xin, "encoder.conv_in", cur, h, w, h, w)
+        st = self._stats(cur)
         in_mult = (1,) + tuple(cfg.ch_mult)
         bi = cfg.ch
         for lvl in range(nres):
             bi, bo = cfg.ch * in_mult[lvl], cfg.ch * cfg.ch_mult[lvl]
+            down = lvl != nres - 1
             for b in range(cfg.num_res_blocks):
-                cur = self._resnet(f"encoder.down.{lvl}.block.{b}.", cur, bi, bo, h, w)
+                # the downsample conv reads the level's last output without a GroupNorm: no table for it
+                cur, st = self._resnet(f"encoder.down.{lvl}.block.{b}.", cur, st, bi, bo, h, w,
+                                       stats=not (down and b == cfg.num_res_blocks - 1))
                 bi = bo
-            if lvl != nres - 1:   # Downsample: F.pad (0,1,0,1) + conv3x3 stride 2 pad 0 (model.py:84-88)
+            if down:   # Downsample: F.pad (0,1,0,1) + conv3x3 stride 2 pad 0 (model.py:84-88)
                 out = self._nxt(n * (h // 2) * (w // 2), bi)
                 self._conv(cur, f"encoder.down.{lvl}.downsample.conv", out, h // 2, w // 2, h, w, stride=2, pad_lo=0)
                 cur, h, w = out, h // 2, w // 2
-        cur = self._resnet("encoder.mid.block_1.", cur, bi, bi, h, w)
-        cur = self._attn("encoder.mid.attn_1.", cur, bi, h, w)
-        cur = self._resnet("encoder.mid.block_2.", cur, bi, bi, h, w)
+                st = self._stats(cur)
+        cur, st = self._resnet("encoder.mid.block_1.", cur, st, bi, bi, h, w)
+        cur, st = self._attn("encoder.mid.attn_1.", cur, st, bi, h, w)
+        cur, st = self._resnet("encoder.mid.block_2.", cur, st, bi, bi, h, w)
         M = n * h * w
         g = A.want("gn", M, bi)
-        self._gn(cur, "encoder.norm_out", h * w, g)
+        self._gn(cur, st, "encoder.norm_out", h * w, g)
         mom = A.want("h", M, 64)     # conv_out output, padded to 64 channels so quant_conv (1x1) sees one K segment
         self._conv(g, "encoder.conv_out", mom, h, w, h, w)
         self.out = A.want("moments", M, COUT_PAD)
@@ -235,26 +229,29 @@ class _VAEPlan:
         bi = cfg.ch * cfg.ch_mult[-1]
         cur = self._nxt(n * h * w, bi)
         self._conv(zq, "decoder.conv_in", cur, h, w, h, w)
-        cur = resnet("decoder.mid.block_1.", cur, bi, bi, h, w)
-        cur = self._attn("decoder.mid.attn_1.", cur, bi, h, w)
-        cur = resnet("decoder.mid.block_2.", cur, bi, bi, h, w)
+        st = self._stats(cur)
+        cur, st = resnet("decoder.mid.block_1.", cur, st, bi, bi, h, w)
+        cur, st = self._attn("decoder.mid.attn_1.", cur, st, bi, h, w)
+        cur, st = resnet("decoder.mid.block_2.", cur, st, bi, bi, h, w)
         for lvl in reversed(range(nres)):
             bo = cfg.ch * cfg.ch_mult[lvl]
             for b in range(cfg.num_res_blocks + 1):
-                cur = resnet(f"decoder.up.{lvl}.block.{b}.", cur, bi, bo, h, w)
+                # the upsample conv reads the level's last output without a GroupNorm: no table for it
+                cur, st = resnet(f"decoder.up.{lvl}.block.{b}.", cur, st, bi, bo, h, w,
+                                 stats=not (lvl != 0 and b == cfg.num_res_blocks))
                 bi = bo
             if lvl != 0:          # Upsample: nearest x2 + conv3x3 (model.py:67-71), fused into the gather
                 out = self._nxt(n * 4 * h * w, bi)
                 parity, ub = self.P[f"decoder.up.{lvl}.upsample.conv"]
-                trk = self._track(out, bi, h * w)               # one statistics table for the four parity launches
                 for (py, px), (Wt, shifts) in parity.items():   # nearest-x2 + conv3x3 == 4 parity-class 2x2 convs
                     self._gemm(lambda shifts=shifts, cur=cur: [ops.SegSpec(cur.t, dy=sy, dx=sx) for sy, sx in shifts], Wt,
                                out, n * h * w, mode=ops.ROWS_CONV2D,
-                               geom=dict(Ho=h, Wo=w, Hs=h, Ws=w, out_up=1, out_py=py, out_px=px), bias=ub, **trk)
+                               geom=dict(Ho=h, Wo=w, Hs=h, Ws=w, out_up=1, out_py=py, out_px=px), bias=ub)
                 cur, h, w = out, 2 * h, 2 * w
+                st = self._stats(cur)                           # one table, after the four parity launches
         M = n * h * w
         g = A.want("gn", M, bi)
-        self._gn(cur, "decoder.norm_out", h * w, g)
+        self._gn(cur, st, "decoder.norm_out", h * w, g)
         self.out = A.want("img", M, COUT_PAD)
         if not video:
             self._conv(g, "decoder.conv_out", self.out, h, w, h, w)

@@ -94,17 +94,6 @@ typedef struct {
   float alpha;
   void* out;                /* fp16 [M, out_ld]                                                        */
   int32_t out_ld;
-  /* GroupNorm statistics of the OUTPUT tensor, for the GroupNorm that consumes it (openaimodel.py:257-261,292-305): after
-   * the GEMM has stored the tensor, the same call runs hi3d_groupnorm_unit_stats over it (the last of an up-conv's four
-   * parity-class launches does, once the tensor is complete), with that function's ordering guarantees.
-   * gn_stats: fp32 [n_images, N / gn_unit, 2], (sum, sum of squares) of the stored fp16 values per image and per unit of
-   * gn_unit consecutive channels, ACCUMULATED (the caller zeroes it); image of a row = (row of the Ho x Wo / HW GEMM grid) /
-   * gn_rows.  Units, not the 32 groups, because a
-   * consumer may normalise the channel concat of two tensors (video_model.py:491) whose groups straddle the boundary;
-   * gn_unit divides every channels-per-group value of the network (model_channels / 32).  NULL = off. */
-  float* gn_stats;
-  int32_t gn_unit;
-  int32_t gn_rows;
 } hi3d_gemm_params;
 
 int hi3d_gemm(const hi3d_gemm_params* p, void* stream);
@@ -132,9 +121,10 @@ int hi3d_gemm_tc5_set_epilogue_warps(int warps);
  * model.py:52-55; eps 1e-6) and the following nn.SiLU / x*sigmoid(x).  Output y: fp16 [rows, C1+C2].
  *
  * Statistics travel as unit tables: fp32 [n_images, C/unit, 2] = (sum, sum of squares) per image and per `unit` consecutive
- * channels, accumulated (zero the table first).  The GEMM that produces a tensor fills its table (hi3d_gemm_params::gn_stats)
- * through hi3d_groupnorm_unit_stats, which computes the table of an existing tensor.  unit must divide C1, C2 and C/32, with
- * at most 256 units per tensor.
+ * channels, accumulated (zero the table first).  A producer's table is made by calling hi3d_groupnorm_unit_stats on its
+ * output after it (after the last of an up-conv's four parity-class launches, once the tensor is complete).  Units, not the
+ * 32 groups, because a consumer may normalise the channel concat of two tensors (video_model.py:491) whose groups straddle
+ * the boundary.  unit must divide C1, C2 and C/32, with at most 256 units per tensor.
  *
  * Reproducibility: hi3d_groupnorm_unit_stats and hi3d_groupnorm_group_sums use no float atomics and sum in a fixed order.
  *  - The same input gives the same table bits on every call.
@@ -292,7 +282,7 @@ int hi3d_dpt_stem_rows(const void* img, int img_is_fp32, int n, int H, int W, in
 int hi3d_maxpool3x3s2_same(const void* x, int n, int H, int W, int C, void* y, void* stream);
 /* y = [ReLU](GroupNorm32(x) + addend) in one pass, for the bottlenecks of BiT (timm ResNetV2 Bottleneck, preact=False:
  * act3(norm3(conv3) + shortcut)) and its stem's GroupNorm + ReLU.  x fp16 [n_images * rows_per_image, C]; its group statistics
- * come from `stats`, the hi3d_gemm_params::gn_stats table of the GEMM that wrote x (fp32 [n_images, C / unit, 2]); gamma /
+ * come from `stats`, the hi3d_groupnorm_unit_stats table of x (fp32 [n_images, C / unit, 2]); gamma /
  * beta fp32 [C].  The addend is NULL, a raw fp16 tensor of x's shape (add_stats NULL), or a second GroupNorm-affine tensor
  * GroupNorm32(add) with its own table and parameters (the projection shortcut of a stage's first block).  Statistics are
  * combined in fp64; the arithmetic is fp32 and y is rounded once.  y may be haloed: image i starts at row

@@ -162,7 +162,7 @@ def test_upsample_conv_as_parity_convs(engine, n, ci, co, hs):
     close(out.view(n, 2 * hs, 2 * hs, co).permute(0, 3, 1, 2), ref, rtol=4e-3, name=f"upconv parity {engine}")
 
 
-# ---- GroupNorm statistics from the epilogue (hi3d_gemm_params::gn_stats) and the one-launch apply that consumes them ------
+# ---- GroupNorm statistics of a GEMM's output (groupnorm_unit_stats after it) and the one-launch apply that consumes them --
 def _unit_sums(out2d, n_img, rows, unit):
     """(sum, sumsq) per image and per `unit` channels of the STORED fp16 tensor."""
     o = out2d.float().view(n_img, rows, -1, unit)
@@ -177,7 +177,7 @@ def _close_stats(got, ref, name):
 
 @pytest.mark.parametrize("engine", ["tc5", "mma"])
 @pytest.mark.parametrize("n,ci,co,hh,unit", [(4, 64, 320, 32, 10), (8, 64, 64, 8, 2), (32, 64, 64, 4, 2), (2, 128, 640, 16, 10)])
-def test_gemm_epilogue_gn_stats_conv(engine, n, ci, co, hh, unit):
+def test_gemm_then_unit_stats_conv(engine, n, ci, co, hh, unit):
     x, w, b = rnd(n, ci, hh, hh), rnd(co, ci, 3, 3, scale=(9 * ci) ** -0.5), rnd(co, scale=0.1)
     res = rnd(n * hh * hh, co, seed=9).to(H)
     xh = nhwc(x)
@@ -185,19 +185,21 @@ def test_gemm_epilogue_gn_stats_conv(engine, n, ci, co, hh, unit):
     out = torch.zeros(M, co, dtype=H, device=DEV)
     stats = torch.zeros(n, co // unit, 2, device=DEV)
     ops.Gemm(ops.conv_taps([xh]), pack.pack_conv2d(w), out, M, mode=ops.ROWS_CONV2D, geom=dict(Ho=hh, Wo=hh, Hs=hh, Ws=hh),
-             bias=b, residual=res, engine=engine, gn_stats=stats.view(-1), gn_unit=unit, gn_rows=hh * hh)()
+             bias=b, residual=res, engine=engine)()
+    ops.groupnorm_unit_stats(out, n, hh * hh, unit, stats.view(-1))
     ref = F.conv2d(xh.permute(0, 3, 1, 2).float(), w.to(H).float(), b, padding=1)
     close(out.view(n, hh, hh, co).permute(0, 3, 1, 2), ref.to(H).float() + res.view(n, hh, hh, co).permute(0, 3, 1, 2).float(),
           name="conv + residual (with stats)")
-    _close_stats(stats, _unit_sums(out, n, hh * hh, unit), f"epilogue stats conv {engine}")
+    _close_stats(stats, _unit_sums(out, n, hh * hh, unit), f"unit stats conv {engine}")
     # accumulate semantics: a second launch adds
     ops.Gemm(ops.conv_taps([xh]), pack.pack_conv2d(w), out, M, mode=ops.ROWS_CONV2D, geom=dict(Ho=hh, Wo=hh, Hs=hh, Ws=hh),
-             bias=b, residual=res, engine=engine, gn_stats=stats.view(-1), gn_unit=unit, gn_rows=hh * hh)()
-    _close_stats(stats, 2 * _unit_sums(out, n, hh * hh, unit), f"epilogue stats accumulate {engine}")
+             bias=b, residual=res, engine=engine)()
+    ops.groupnorm_unit_stats(out, n, hh * hh, unit, stats.view(-1))
+    _close_stats(stats, 2 * _unit_sums(out, n, hh * hh, unit), f"unit stats accumulate {engine}")
 
 
 @pytest.mark.parametrize("pair", [-1, 1])
-def test_gemm_epilogue_gn_stats_temporal_plain_upconv(pair):
+def test_gemm_then_unit_stats_temporal_plain_upconv(pair):
     lib = __import__("hi3d_official_b200._native", fromlist=["x"]).load()
     lib.hi3d_gemm_tc5_set_pair_mode(pair)
     try:
@@ -210,16 +212,18 @@ def test_gemm_epilogue_gn_stats_temporal_plain_upconv(pair):
             out = torch.zeros(M, co, dtype=H, device=DEV)
             stats = torch.zeros(b_ * T, co // unit, 2, device=DEV)
             ops.Gemm(ops.temporal_taps(xh), pack.pack_conv3d_t(w), out, M, mode=ops.ROWS_TEMPORAL, geom=dict(Ho=hw, Wo=1, T=T),
-                     engine="tc5", gn_stats=stats.view(-1), gn_unit=unit, gn_rows=hw)()
-            _close_stats(stats, _unit_sums(out, b_ * T, hw, unit), f"epilogue stats temporal hw={hw}")
+                     engine="tc5")()
+            ops.groupnorm_unit_stats(out, b_ * T, hw, unit, stats.view(-1))
+            _close_stats(stats, _unit_sums(out, b_ * T, hw, unit), f"unit stats temporal hw={hw}")
         # plain rows (proj_out-like), ragged last tile, images of 100 rows
         M, K, N, rows, unit = 700, 320, 320, 100, 10
         a, w = rnd(M, K).to(H), rnd(N, K, scale=K ** -0.5).to(H)
         out = torch.zeros(M, N, dtype=H, device=DEV)
         stats = torch.zeros(M // rows, N // unit, 2, device=DEV)
-        ops.Gemm([ops.SegSpec(a)], w, out, M, engine="tc5", gn_stats=stats.view(-1), gn_unit=unit, gn_rows=rows)()
-        _close_stats(stats, _unit_sums(out, M // rows, rows, unit), "epilogue stats plain")
-        # nearest x2 + conv as four parity launches accumulating into one table
+        ops.Gemm([ops.SegSpec(a)], w, out, M, engine="tc5")()
+        ops.groupnorm_unit_stats(out, M // rows, rows, unit, stats.view(-1))
+        _close_stats(stats, _unit_sums(out, M // rows, rows, unit), "unit stats plain")
+        # nearest x2 + conv as four parity launches into one tensor, one table over its 4 hs^2 rows per image
         n, ci, co, hs, unit = 2, 64, 64, 16, 2
         x, w = rnd(n, ci, hs, hs), rnd(co, ci, 3, 3, scale=(9 * ci) ** -0.5)
         xh = nhwc(x)
@@ -227,9 +231,9 @@ def test_gemm_epilogue_gn_stats_temporal_plain_upconv(pair):
         stats = torch.zeros(n, co // unit, 2, device=DEV)
         for (py, px), (Wt, shifts) in pack.pack_upconv_parity(w).items():
             ops.Gemm([ops.SegSpec(xh, dy=sy, dx=sx) for sy, sx in shifts], Wt, out, n * hs * hs, mode=ops.ROWS_CONV2D,
-                     geom=dict(Ho=hs, Wo=hs, Hs=hs, Ws=hs, out_up=1, out_py=py, out_px=px), engine="tc5",
-                     gn_stats=stats.view(-1), gn_unit=unit, gn_rows=hs * hs)()
-        _close_stats(stats, _unit_sums(out, n, 4 * hs * hs, unit), "epilogue stats upconv")
+                     geom=dict(Ho=hs, Wo=hs, Hs=hs, Ws=hs, out_up=1, out_py=py, out_px=px), engine="tc5")()
+        ops.groupnorm_unit_stats(out, n, 4 * hs * hs, unit, stats.view(-1))
+        _close_stats(stats, _unit_sums(out, n, 4 * hs * hs, unit), "unit stats upconv")
     finally:
         lib.hi3d_gemm_tc5_set_pair_mode(-1)
 

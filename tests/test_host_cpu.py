@@ -13,14 +13,14 @@ from oracle import hi3d_oracle as O
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def test_library_exports_every_declared_symbol():
+def test_library_abi4_exports_every_declared_symbol():
     lib = _native.load()
     hdr = open(os.path.join(ROOT, "include", "hi3d_b200.h")).read()
     declared = set(re.findall(r"\b(hi3d_[a-z0-9_]+)\s*\(", hdr))
     assert declared == set(_native.EXPORTS), declared ^ set(_native.EXPORTS)
     for s in declared:
         assert hasattr(lib, s)
-    assert lib.hi3d_abi_version() == 3
+    assert lib.hi3d_abi_version() == 4
     # parameter-block layout must match the C struct: 17 ints (+4 pad), 24 segs of 32 bytes, then the tail
     assert _native.GemmParams.seg.offset == 72 and _native.Seg.__dict__["dt"].offset == 28
     import ctypes

@@ -279,7 +279,7 @@ def _tc5_tiles(Tl, HW, N):
     pytest.param("mma", 2, 4, 4, 16, 640, id="tc5-forwards-to-mma-Tl4-hw16-c640"),
     pytest.param("mma", 2, 3, 5, 100, 320, id="tc5-forwards-to-mma-Tl3-hw100-c320"),
 ])
-def test_sharded_temporal_conv_over_halo(pair_mode, engine, pair, path, B, Tl, world, HW, Cc):
+def test_sharded_temporal_conv_over_halo_then_unit_stats(pair_mode, engine, pair, path, B, Tl, world, HW, Cc):
     assert _tc5_tiles(Tl, HW, Cc) == (path == "tc5"), "case id names the wrong engine path"
     pair_mode(pair)
     gw = _GnWorld(B, Tl, world, Cc, HW, seed=11)
@@ -305,20 +305,21 @@ def test_sharded_temporal_conv_over_halo(pair_mode, engine, pair, path, B, Tl, w
         out = _nans(M, Cc)
         st = torch.zeros(B * Tl, Cc // GN_UNIT, 2, device=DEV)
         ops.Gemm(ops.temporal_taps(gw.gh[r]), wp, out, M, mode=ops.ROWS_TEMPORAL, geom=geo, bias=bias,
-                 rowbias=emb[:, sl].reshape(B * Tl, Cc), rb_div=HW, rb_mod=B * Tl, engine=engine,
-                 gn_stats=st.view(-1), gn_unit=GN_UNIT, gn_rows=HW)()
+                 rowbias=emb[:, sl].reshape(B * Tl, Cc), rb_div=HW, rb_mod=B * Tl, engine=engine)()
+        ops.groupnorm_unit_stats(out, B * Tl, HW, GN_UNIT, st.view(-1))
         ref = cr + emb[:, sl].float().repeat_interleave(HW, 1).reshape(M, Cc)
         _check(out, ref, f"temporal conv + rowbias rank {r} {tag}")
-        _close_stats(st, _unit_sums(out, B * Tl, HW, GN_UNIT), f"gn_stats rank {r} {tag}")
+        _close_stats(st, _unit_sums(out, B * Tl, HW, GN_UNIT), f"unit stats rank {r} {tag}")
         # 2. bias + residual + alpha blend (the second conv: out = alpha x + (1 - alpha) (x + conv))
         res = xs[:, sl].reshape(M, Cc)
         out = _nans(M, Cc)
         st = torch.zeros(B * Tl, Cc // GN_UNIT, 2, device=DEV)
         ops.Gemm(ops.temporal_taps(gw.gh[r]), wp, out, M, mode=ops.ROWS_TEMPORAL, geom=geo, bias=bias, residual=res,
-                 blend_x=res, alpha=alpha, engine=engine, gn_stats=st.view(-1), gn_unit=GN_UNIT, gn_rows=HW)()
+                 blend_x=res, alpha=alpha, engine=engine)()
+        ops.groupnorm_unit_stats(out, B * Tl, HW, GN_UNIT, st.view(-1))
         ref = alpha * res.float() + (1 - alpha) * (cr.to(H).float() + res.float())
         _check(out, ref, f"temporal conv + residual + blend rank {r} {tag}")
-        _close_stats(st, _unit_sums(out, B * Tl, HW, GN_UNIT), f"gn_stats (blend) rank {r} {tag}")
+        _close_stats(st, _unit_sums(out, B * Tl, HW, GN_UNIT), f"unit stats (blend) rank {r} {tag}")
 
 
 # ======================================================================================================================
