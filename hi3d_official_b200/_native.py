@@ -50,9 +50,14 @@ _SIGS = {
     "hi3d_gemm_tc5": (C.c_int, [C.POINTER(GemmParams), C.c_void_p]),
     "hi3d_gemm_tc5_set_pair_mode": (C.c_int, [C.c_int]),
     "hi3d_gemm_tc5_set_epilogue_warps": (C.c_int, [C.c_int]),
+    "hi3d_gemm_tc5_fp8": (C.c_int, [C.POINTER(GemmParams), C.c_void_p, C.c_int, C.c_void_p]),
+    "hi3d_gemm_tc5_fp8_covers": (C.c_int, [C.POINTER(GemmParams)]),
     "hi3d_groupnorm_apply_stats": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int,
                                              C.c_int64, C.c_int, C.c_int64, C.c_void_p, C.c_void_p, C.c_float, C.c_int,
                                              C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
+    "hi3d_groupnorm_apply_stats_fp8": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int,
+                                                 C.c_int, C.c_int64, C.c_int, C.c_int64, C.c_void_p, C.c_void_p, C.c_float,
+                                                 C.c_int, C.c_void_p, C.c_void_p]),
     "hi3d_groupnorm_unit_stats": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_void_p, C.c_void_p]),
     "hi3d_groupnorm_group_sums": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                             C.c_void_p]),
@@ -61,6 +66,8 @@ _SIGS = {
                                             C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),
     "hi3d_layernorm": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_void_p,
                                  C.c_void_p, C.c_float, C.c_void_p, C.c_void_p]),
+    "hi3d_layernorm_fp8": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_void_p,
+                                     C.c_void_p, C.c_float, C.c_void_p, C.c_void_p]),
     "hi3d_attention_d64": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_void_p]),
     "hi3d_attention_d64_tc5": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_void_p]),
     "hi3d_attention_tc5_set_exp_emulation": (C.c_int, [C.c_int]),

@@ -106,6 +106,19 @@ struct alignas(16) Half8 {
   }
 };
 
+// Eight fp16 values -> eight e4m3 bytes (one 8-byte store), cvt.rn.satfinite.e4m3x2.f16x2 per pair: round to nearest even, and
+// finite values beyond +-448 saturate.  So every e4m3 output equals clamp(fp16 output, -448, 448) cast to e4m3.
+HI3D_DEVINL uint2 half8_to_e4m3(const Half8& v) {
+  uint32_t w[4];
+#pragma unroll
+  for (int q = 0; q < 4; q++) {
+    uint16_t r;
+    asm("cvt.rn.satfinite.e4m3x2.f16x2 %0, %1;\n" : "=h"(r) : "r"(*reinterpret_cast<const uint32_t*>(&v.h[q])));
+    w[q] = r;                                   // low byte = the pair's .x
+  }
+  return make_uint2(w[0] | (w[1] << 16), w[2] | (w[3] << 16));
+}
+
 // HI3D_ACT_GELU / HI3D_ACT_QUICKGELU (the CLIP towers' MLP activations) and HI3D_ACT_RELU (the DPT depth tower's convs) on
 // eight staged fp16 GEMM outputs.  Both GEMM engines apply them in their store pass, on the fp16 tile, before the residual:
 // the register pass that produces the tile (bias, SiLU, GEGLU) is shared by every UNet GEMM, and code added to that unrolled

@@ -17,7 +17,11 @@
 // one CTA that share every B tile -- half the B bytes from L2 per output row, for long-K shapes -- and is built for
 // BN <= 128 (the register budget of 640 threads).  The producer hands its registers to the MMA warpgroups (setmaxnreg):
 // a 64 x 256 fp32 accumulator is 128 registers per thread.
+// The kernel is templated on the operand type: hi3d_gemm_tc5 runs fp16 operands and hi3d_gemm_tc5_fp8 e4m3 ones (wgmma k32,
+// SWIZZLE_64B stages, a per-column weight scale on the fp32 accumulator and an optional e4m3 output); the producer, the row
+// mappings and the epilogue are shared.
 #include <cuda.h>
+#include <cuda_fp8.h>
 #include <stdlib.h>
 #include <string.h>
 
@@ -30,9 +34,22 @@ int validate_gemm(const hi3d_gemm_params* p, const char* who);
 constexpr int T5_BM = 128;
 constexpr int T5_BK = 64;
 constexpr int T5_MAX_MAPS = 4;
-constexpr int T5_MAX_STAGES = 8;
-constexpr int T5_A_BYTES = T5_BM * 128;
 constexpr int T5_SMEM_BUDGET = 200 * 1024;
+
+// Operand types.  fp16: a stage holds 64-element K rows of 128 bytes under SWIZZLE_128B, four k16 MMAs per stage.  e4m3: 64-element
+// K rows of 64 bytes under SWIZZLE_64B (segment channel counts are multiples of 64, not of 128), two k32 MMAs per stage; the
+// stages are half the bytes, so twice as many fit the same shared memory.
+template <typename Op> struct T5Op;
+template <> struct T5Op<__half> {
+  static constexpr int ROW = 128, MAX_STAGES = 8;
+  static constexpr CUtensorMapDataType DT = CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  static constexpr CUtensorMapSwizzle SW = CU_TENSOR_MAP_SWIZZLE_128B;
+};
+template <> struct T5Op<__nv_fp8_e4m3> {
+  static constexpr int ROW = 64, MAX_STAGES = 16;
+  static constexpr CUtensorMapDataType DT = CU_TENSOR_MAP_DATA_TYPE_UINT8;
+  static constexpr CUtensorMapSwizzle SW = CU_TENSOR_MAP_SWIZZLE_64B;
+};
 
 struct T5Seg {
   int map;       // index into amap[]
@@ -65,6 +82,8 @@ struct T5Params {
   float alpha;
   __half* out;
   int out_ld;
+  const float* w_scale;   // e4m3 operands: per-column dequantisation scale of W, applied to the accumulator first
+  int out_fp8;            // e4m3 operands: 1 -> out is e4m3 [M, out_ld]
 };
 
 struct T5Tile {
@@ -94,17 +113,20 @@ HI3D_DEVINL long long t5_row(const T5Params& p, int mt, const T5Tile& o, int r) 
   return ((long long)n * p.Ho + y) * p.Wo + x;
 }
 
-template <int BN, int NT>
+template <int BN, int NT, typename Op>
 __global__ void __launch_bounds__(128 + 256 * NT, 1) gemm_tc5_kernel(const __grid_constant__ T5Params p) {
+  constexpr bool FP8 = sizeof(Op) == 1;
+  constexpr int ROW = T5Op<Op>::ROW;             // bytes of one 64-element K row of a stage
+  constexpr int A_BYTES = T5_BM * ROW;
   constexpr int MMA_THREADS = 256 * NT;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;          // SWIZZLE_128B atoms need 1024-byte alignment
   uint8_t* smem = smem_raw + (base - raw);
   const int STAGES = p.stages;
-  constexpr uint32_t stage_bytes = NT * T5_A_BYTES + BN * 128;
+  constexpr uint32_t stage_bytes = NT * A_BYTES + BN * ROW;
   const uint32_t bar_full = base + STAGES * stage_bytes;   // STAGES x 8
-  const uint32_t bar_empty = bar_full + 8 * T5_MAX_STAGES;
+  const uint32_t bar_empty = bar_full + 8 * T5Op<Op>::MAX_STAGES;
 
   const int tid = threadIdx.x, lane = tid & 31;
   const int wg = __shfl_sync(0xffffffffu, tid >> 7, 0);    // provably warp-uniform role index
@@ -136,13 +158,13 @@ __global__ void __launch_bounds__(128 + 256 * NT, 1) gemm_tc5_kernel(const __gri
       for (int kt = 0; kt < KT; kt++) {
         mbar_wait(bar_empty + 8 * s, ph ^ 1);
         if (lane == 0) {
-          const uint32_t sB = base + s * stage_bytes + NT * T5_A_BYTES;
+          const uint32_t sB = base + s * stage_bytes + NT * A_BYTES;
           const uint32_t full = bar_full + 8 * s;
           const int c = sg.c_off + so;
           mbar_expect_tx(full, stage_bytes);
           // a second row tile past the last one loads out of bounds (zeros) and stores nothing
           for (int t = 0; t < NT; t++) {
-            const uint32_t sA = base + s * stage_bytes + t * T5_A_BYTES;
+            const uint32_t sA = base + s * stage_bytes + t * A_BYTES;
             if (p.mode == HI3D_ROWS_PLAIN)
               tma_load_2d(sA, am, full, c, (mt0 + t) * T5_BM);
             else if (p.mode == HI3D_ROWS_CONV2D)
@@ -175,13 +197,20 @@ __global__ void __launch_bounds__(128 + 256 * NT, 1) gemm_tc5_kernel(const __gri
     uint32_t s = 0, ph = 0, ps = 0;
     for (int kt = 0; kt < KT; kt++) {
       mbar_wait(bar_full + 8 * s, ph);
-      const uint32_t sA = base + s * stage_bytes + cw * 64 * 128;
-      const uint32_t sB = base + s * stage_bytes + NT * T5_A_BYTES;
-      const uint64_t ad = gmma_desc_sw128(sA), bd = gmma_desc_sw128(sB);
+      const uint32_t sA = base + s * stage_bytes + cw * 64 * ROW;
+      const uint32_t sB = base + s * stage_bytes + NT * A_BYTES;
       wgmma_fence();
+      if constexpr (FP8) {
+        const uint64_t ad = gmma_desc_sw64(sA), bd = gmma_desc_sw64(sB);
 #pragma unroll
-      for (int k = 0; k < T5_BK / 16; k++)   // +32 bytes along K inside the 128-byte swizzle atom
-        wgmma_ss<BN>(acc, ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), (kt | k) ? 1 : 0);
+        for (int k = 0; k < T5_BK / 32; k++)   // +32 bytes along K inside the 64-byte swizzle atom
+          wgmma_ss_e4m3<BN>(acc, ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), (kt | k) ? 1 : 0);
+      } else {
+        const uint64_t ad = gmma_desc_sw128(sA), bd = gmma_desc_sw128(sB);
+#pragma unroll
+        for (int k = 0; k < T5_BK / 16; k++)   // +32 bytes along K inside the 128-byte swizzle atom
+          wgmma_ss<BN>(acc, ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), (kt | k) ? 1 : 0);
+      }
       wgmma_commit();
       // keep one k-block of MMAs in flight: the previous one has retired, its stage goes back to the producer
       wgmma_wait<1>();
@@ -213,6 +242,11 @@ __global__ void __launch_bounds__(128 + 256 * NT, 1) gemm_tc5_kernel(const __gri
       const int n = n0 + cl;
       float v0 = acc[4 * j + 2 * hh], v1 = acc[4 * j + 2 * hh + 1];
       if (n < p.N) {
+        if constexpr (FP8) {
+          const float2 ws = __ldg(reinterpret_cast<const float2*>(p.w_scale + n));
+          v0 *= ws.x;
+          v1 *= ws.y;
+        }
         if (p.bias != nullptr) {
           v0 += __ldg(p.bias + n);
           v1 += __ldg(p.bias + n + 1);
@@ -274,6 +308,12 @@ __global__ void __launch_bounds__(128 + 256 * NT, 1) gemm_tc5_kernel(const __gri
         v.h[q] = __floats2half2_rn(al * b.x + be * a.x, al * b.y + be * a.y);
       }
     }
+    if constexpr (FP8) {
+      if (p.out_fp8) {
+        *reinterpret_cast<uint2*>(reinterpret_cast<uint8_t*>(p.out) + mo * p.out_ld + nc) = half8_to_e4m3(v);
+        continue;
+      }
+    }
     *reinterpret_cast<Half8*>(p.out + mo * p.out_ld + nc) = v;
   }
 }
@@ -295,12 +335,12 @@ static EncodeTiledFn get_encode() {
 }
 
 int encode_map(CUtensorMap* m, const void* ptr, int rank, const cuuint64_t* dims, const cuuint64_t* strides_bytes,
-               const cuuint32_t* box, const cuuint32_t* elem_strides, CUtensorMapSwizzle swizzle) {
+               const cuuint32_t* box, const cuuint32_t* elem_strides, CUtensorMapSwizzle swizzle, CUtensorMapDataType dtype) {
   EncodeTiledFn enc = get_encode();
   if (!enc) { set_error("hi3d_gemm_tc5: cuTensorMapEncodeTiled entry point unavailable"); return -1; }
   cuuint32_t estr[5] = {1, 1, 1, 1, 1};
   if (elem_strides) for (int i = 0; i < rank; i++) estr[i] = elem_strides[i];
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, (cuuint32_t)rank, const_cast<void*>(ptr), dims, strides_bytes, box,
+  CUresult r = enc(m, dtype, (cuuint32_t)rank, const_cast<void*>(ptr), dims, strides_bytes, box,
                    estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
@@ -324,11 +364,11 @@ static void read_env_once() {
   if (g_ew_mode != 8 && g_ew_mode != 16) g_ew_mode = -1;
 }
 
-template <int BN, int NT>
+template <int BN, int NT, typename Op>
 static int launch_tc5(const T5Params& tp, int grid, int smem, cudaStream_t st) {
   static bool attr_done[HI3D_MAX_DEVICES];
-  if (ensure_dyn_smem(gemm_tc5_kernel<BN, NT>, smem, attr_done, "hi3d_gemm_tc5")) return -1;
-  gemm_tc5_kernel<BN, NT><<<grid, 128 + 256 * NT, smem, st>>>(tp);
+  if (ensure_dyn_smem(gemm_tc5_kernel<BN, NT, Op>, smem, attr_done, "hi3d_gemm_tc5")) return -1;
+  gemm_tc5_kernel<BN, NT, Op><<<grid, 128 + 256 * NT, smem, st>>>(tp);
   return check_launch("hi3d_gemm_tc5");
 }
 
@@ -350,18 +390,15 @@ extern "C" int hi3d_gemm_tc5_set_epilogue_warps(int warps) {
   return 0;
 }
 
-extern "C" int hi3d_gemm_tc5(const hi3d_gemm_params* p, void* stream) {
-  int rc = validate_gemm(p, "hi3d_gemm_tc5");
-  if (rc) return rc;
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  // ---- geometry this engine covers; everything else goes to the mma.sync engine (same results) ----
-  T5Params tp;
+// The tiling of one GEMM on this engine, from its geometry alone: tile -> rows mapping, row tiles, and the distinct A sources
+// (srcs / lds, T5_MAX_MAPS entries) that become tensor maps.  False when the engine does not cover the geometry.
+static bool tc5_geometry(const hi3d_gemm_params* p, T5Params& tp, int& m_tiles, const void** srcs, int* lds, int& nmaps) {
   memset(&tp, 0, sizeof(tp));
   tp.M = p->M; tp.N = p->N; tp.K = p->K; tp.mode = p->mode; tp.nseg = p->nseg;
   tp.cstride = (p->mode == HI3D_ROWS_CONV2D) ? p->stride : 1;
   tp.out_up = p->out_up; tp.out_py = p->out_py; tp.out_px = p->out_px;
   tp.t_off = p->t_off;
-  int m_tiles = 0;
+  m_tiles = 0;
   bool ok = (p->N >= 32) && (p->N % 8 == 0);
   ok = ok && (p->rowbias == nullptr || ((uintptr_t)p->rowbias % 4 == 0 && p->rb_ld % 2 == 0));
   if (p->mode == HI3D_ROWS_PLAIN) {
@@ -391,9 +428,7 @@ extern "C" int hi3d_gemm_tc5(const hi3d_gemm_params* p, void* stream) {
     m_tiles = ok ? tp.tiles_x * tp.tiles_y * B : 0;
   }
   // distinct A sources -> tensor maps
-  const void* srcs[T5_MAX_MAPS];
-  int lds[T5_MAX_MAPS];
-  int nmaps = 0;
+  nmaps = 0;
   for (int i = 0; ok && i < p->nseg; i++) {
     const hi3d_seg& s = p->seg[i];
     int mi = -1;
@@ -406,7 +441,36 @@ extern "C" int hi3d_gemm_tc5(const hi3d_gemm_params* p, void* stream) {
     tp.seg[i].map = mi; tp.seg[i].c_off = s.c_off; tp.seg[i].C = s.C;
     tp.seg[i].dy = s.dy; tp.seg[i].dx = s.dx; tp.seg[i].dt = s.dt;
   }
-  if (!ok || m_tiles <= 0) return hi3d_gemm(p, stream);
+  return ok && m_tiles > 0;
+}
+
+// One GEMM on the engine, with fp16 or e4m3 operands.  fp16: geometries the engine does not cover go to the mma.sync engine
+// (same results).  e4m3: there is no other engine, so such a geometry is an error.
+template <typename Op>
+static int tc5_gemm(const hi3d_gemm_params* p, const float* w_scale, int out_fp8, void* stream, const char* who) {
+  constexpr bool FP8 = sizeof(Op) == 1;
+  constexpr int ROW = T5Op<Op>::ROW, ESIZE = sizeof(Op), MAX_STAGES = T5Op<Op>::MAX_STAGES;
+  int rc = validate_gemm(p, who);
+  if (rc) return rc;
+  if (FP8) {
+    // TMA global strides are multiples of 16 bytes
+    for (int i = 0; i < p->nseg; i++)
+      if (p->seg[i].ld % 16) { set_error("%s: e4m3 segment %d has ld %d, not a multiple of 16", who, i, p->seg[i].ld); return -2; }
+    if (w_scale == nullptr || ((uintptr_t)w_scale & 7)) { set_error("%s: w_scale null or misaligned", who); return -2; }
+  }
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  // ---- geometry this engine covers ----
+  T5Params tp;
+  const void* srcs[T5_MAX_MAPS];
+  int lds[T5_MAX_MAPS];
+  int m_tiles = 0, nmaps = 0;
+  const bool ok = tc5_geometry(p, tp, m_tiles, srcs, lds, nmaps);
+  if (!ok) {
+    if (!FP8) return hi3d_gemm(p, stream);
+    set_error("%s: geometry not covered by the e4m3 engine (mode %d, M %d, N %d, Ho %d, Wo %d, T %d, stride %d, ups %d, %d segments)",
+              who, p->mode, p->M, p->N, p->Ho, p->Wo, p->T, p->stride, p->ups, p->nseg);
+    return -2;
+  }
 
   // Tile pairs (NT = 2): two row tiles share each B tile, halving the B bytes per output row; worth it once the main loop
   // dominates (long K) and there are enough tiles to fill the SMs with pairs.  The hooks force either choice.
@@ -429,53 +493,77 @@ extern "C" int hi3d_gemm_tc5(const hi3d_gemm_params* p, void* stream) {
       if (best < 0 || cost < best) { best = cost; BN = cand; }
     }
   }
-  const int stage_bytes = ntile * T5_A_BYTES + BN * 128;
+  const int stage_bytes = ntile * T5_BM * ROW + BN * ROW;
   int stages = T5_SMEM_BUDGET / stage_bytes;
-  if (stages > T5_MAX_STAGES) stages = T5_MAX_STAGES;
+  if (stages > MAX_STAGES) stages = MAX_STAGES;
   tp.stages = stages;
   tp.n_tiles = (p->N + BN - 1) / BN;
   const long long grid = (long long)m_units * tp.n_tiles;
-  if (grid > 2147483647LL) { set_error("hi3d_gemm_tc5: too many tiles"); return -2; }
+  if (grid > 2147483647LL) { set_error("%s: too many tiles", who); return -2; }
 
   for (int j = 0; j < nmaps; j++) {
     const cuuint64_t ld = (cuuint64_t)lds[j];
     if (p->mode == HI3D_ROWS_PLAIN) {
       cuuint64_t dims[2] = {ld, (cuuint64_t)p->M};
-      cuuint64_t str[1] = {ld * 2};
+      cuuint64_t str[1] = {ld * ESIZE};
       cuuint32_t box[2] = {64, 128};
-      if (encode_map(&tp.amap[j], srcs[j], 2, dims, str, box, nullptr)) return -1;
+      if (encode_map(&tp.amap[j], srcs[j], 2, dims, str, box, nullptr, T5Op<Op>::SW, T5Op<Op>::DT)) return -1;
     } else if (p->mode == HI3D_ROWS_CONV2D) {
       cuuint64_t dims[4] = {ld, (cuuint64_t)p->Ws, (cuuint64_t)p->Hs, (cuuint64_t)tp.Nimg};
-      cuuint64_t str[3] = {ld * 2, ld * 2 * p->Ws, ld * 2 * p->Ws * p->Hs};
+      cuuint64_t str[3] = {ld * ESIZE, ld * ESIZE * p->Ws, ld * ESIZE * p->Ws * p->Hs};
       const cuuint32_t cs = (cuuint32_t)tp.cstride;   // stride 2: box spans 2*tw x 2*th input pixels, every 2nd loaded
       cuuint32_t box[4] = {64, (cuuint32_t)tp.tw * cs, (cuuint32_t)tp.th * cs, (cuuint32_t)tp.tn};
       cuuint32_t est[4] = {1, cs, cs, 1};
-      if (encode_map(&tp.amap[j], srcs[j], 4, dims, str, box, est)) return -1;
+      if (encode_map(&tp.amap[j], srcs[j], 4, dims, str, box, est, T5Op<Op>::SW, T5Op<Op>::DT)) return -1;
     } else {
       const cuuint64_t HW = (cuuint64_t)tp.Wo, T = (cuuint64_t)(p->Tin > 0 ? p->Tin : tp.Ho);   // source frames per clip
       cuuint64_t dims[4] = {ld, HW, T, (cuuint64_t)tp.Nimg};
-      cuuint64_t str[3] = {ld * 2, ld * 2 * HW, ld * 2 * HW * T};
+      cuuint64_t str[3] = {ld * ESIZE, ld * ESIZE * HW, ld * ESIZE * HW * T};
       cuuint32_t box[4] = {64, (cuuint32_t)tp.tw, (cuuint32_t)tp.th, 1};
-      if (encode_map(&tp.amap[j], srcs[j], 4, dims, str, box, nullptr)) return -1;
+      if (encode_map(&tp.amap[j], srcs[j], 4, dims, str, box, nullptr, T5Op<Op>::SW, T5Op<Op>::DT)) return -1;
     }
   }
   {
     cuuint64_t dims[2] = {(cuuint64_t)p->K, (cuuint64_t)p->N};
-    cuuint64_t str[1] = {(cuuint64_t)p->K * 2};
+    cuuint64_t str[1] = {(cuuint64_t)p->K * ESIZE};
     cuuint32_t box[2] = {64, (cuuint32_t)BN};
-    if (encode_map(&tp.bmap, p->W, 2, dims, str, box, nullptr)) return -1;
+    if (encode_map(&tp.bmap, p->W, 2, dims, str, box, nullptr, T5Op<Op>::SW, T5Op<Op>::DT)) return -1;
   }
   tp.bias = p->bias; tp.rowbias = (const __half*)p->rowbias; tp.rb_div = p->rb_div; tp.rb_mod = p->rb_mod;
   tp.rb_ld = p->rb_ld; tp.act = p->act; tp.residual = (const __half*)p->residual; tp.res_ld = p->res_ld;
   tp.blend_x = (const __half*)p->blend_x; tp.blend_ld = p->blend_ld; tp.alpha = p->alpha;
   tp.out = (__half*)p->out; tp.out_ld = p->out_ld;
+  tp.w_scale = w_scale; tp.out_fp8 = out_fp8;
 
-  const int smem = stages * stage_bytes + 16 * T5_MAX_STAGES + 1024;
-  if (ntile == 2) return BN == 64 ? launch_tc5<64, 2>(tp, (int)grid, smem, st) : launch_tc5<128, 2>(tp, (int)grid, smem, st);
+  const int smem = stages * stage_bytes + 16 * MAX_STAGES + 1024;
+  if (ntile == 2)
+    return BN == 64 ? launch_tc5<64, 2, Op>(tp, (int)grid, smem, st) : launch_tc5<128, 2, Op>(tp, (int)grid, smem, st);
   switch (BN) {
-    case 64: return launch_tc5<64, 1>(tp, (int)grid, smem, st);
-    case 128: return launch_tc5<128, 1>(tp, (int)grid, smem, st);
-    case 192: return launch_tc5<192, 1>(tp, (int)grid, smem, st);
-    default: return launch_tc5<256, 1>(tp, (int)grid, smem, st);
+    case 64: return launch_tc5<64, 1, Op>(tp, (int)grid, smem, st);
+    case 128: return launch_tc5<128, 1, Op>(tp, (int)grid, smem, st);
+    case 192: return launch_tc5<192, 1, Op>(tp, (int)grid, smem, st);
+    default: return launch_tc5<256, 1, Op>(tp, (int)grid, smem, st);
   }
+}
+
+extern "C" int hi3d_gemm_tc5(const hi3d_gemm_params* p, void* stream) {
+  return tc5_gemm<__half>(p, nullptr, 0, stream, "hi3d_gemm_tc5");
+}
+
+extern "C" int hi3d_gemm_tc5_fp8(const hi3d_gemm_params* p, const float* w_scale, int out_fp8, void* stream) {
+  return tc5_gemm<__nv_fp8_e4m3>(p, w_scale, out_fp8 ? 1 : 0, stream, "hi3d_gemm_tc5_fp8");
+}
+
+extern "C" int hi3d_gemm_tc5_fp8_covers(const hi3d_gemm_params* p) {
+  if (p == nullptr || p->M <= 0 || p->N <= 0 || p->nseg <= 0 || p->nseg > HI3D_MAX_SEGS ||
+      (p->mode == HI3D_ROWS_CONV2D && (p->Ho <= 0 || p->Wo <= 0)) ||
+      (p->mode == HI3D_ROWS_TEMPORAL && (p->Ho <= 0 || p->Wo <= 0 || p->T <= 0))) {
+    set_error("hi3d_gemm_tc5_fp8_covers: bad parameters");
+    return -2;
+  }
+  T5Params tp;
+  const void* srcs[T5_MAX_MAPS];
+  int lds[T5_MAX_MAPS];
+  int m_tiles = 0, nmaps = 0;
+  return tc5_geometry(p, tp, m_tiles, srcs, lds, nmaps) ? 1 : 0;
 }

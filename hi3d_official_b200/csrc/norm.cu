@@ -23,8 +23,9 @@ HI3D_DEVINL Half8 ld_stream(const __half* p) {
 // ---- GroupNorm apply: y = [silu]((x - mean) * rstd * gamma + beta) ----------------------------------
 // grid (row_slabs, n_samples), blockDim = RL * CV.  Statistics: the unit tables stats1 / stats2 when stats1 != NULL, else the
 // per-(sample, group) sums `fin` over `count` elements.
-template <bool HALO>      // HALO = haloed output with peer stores / boundary zero fill (frame-sharded temporal GroupNorm only):
+template <bool HALO,      // HALO = haloed output with peer stores / boundary zero fill (frame-sharded temporal GroupNorm only):
                           // a template so that the dense kernel keeps its 64 registers (2 CTAs per SM)
+          bool OUT8>      // OUT8 = dense e4m3 output: each fp16 result the fp16 kernel would store, converted by half8_to_e4m3
 __global__ void __launch_bounds__(512)
 gn_apply_kernel(const __half* __restrict__ x1, int C1, const __half* __restrict__ x2, int C2, long long rows_per_sample,
                 long long rows_per_cta, const float* __restrict__ fin, double count, float eps,
@@ -110,7 +111,12 @@ gn_apply_kernel(const __half* __restrict__ x1, int C1, const __half* __restrict_
   Half8 zero8;
   zero8.u = make_uint4(0u, 0u, 0u, 0u);
   bool remote = false;
+  uint8_t* yb8 = reinterpret_cast<uint8_t*>(y) + ((long long)n * y_sample_rows + y_row_off) * C + c0;
   auto put = [&](long long rr, const Half8& o) {
+    if constexpr (OUT8) {
+      *reinterpret_cast<uint2*>(yb8 + rr * C) = half8_to_e4m3(o);
+      return;
+    }
     *reinterpret_cast<Half8*>(yb + rr * C) = o;
     if (!HALO) return;
     if (rr < frame_rows) {
@@ -136,7 +142,8 @@ gn_apply_kernel(const __half* __restrict__ x1, int C1, const __half* __restrict_
 
 // ---- LayerNorm: LPR lanes per row (32/LPR rows per warp pass), VPL 16-byte vectors per lane ------------------
 // C = 8 * VPL * LPR exactly (C = 320 -> VPL 5, LPR 8; 640 -> 5 x 16; 1280 -> 5 x 32; 64 -> 1 x 8; 2560 -> 10 x 32).
-template <int VPL, int LPR>
+// OUT8: y is e4m3, each fp16 result the fp16 kernel would store converted by half8_to_e4m3 (both LayerNorm kernels).
+template <int VPL, int LPR, bool OUT8>
 __global__ void __launch_bounds__(256)
 layernorm_kernel(const __half* __restrict__ x, const __half* __restrict__ addvec, int add_div, int add_mod, long long M,
                  int C, const float* __restrict__ gamma, const float* __restrict__ beta, float eps,
@@ -203,13 +210,14 @@ layernorm_kernel(const __half* __restrict__ x, const __half* __restrict__ addvec
         const float2 bt = *reinterpret_cast<const float2*>(beta + c0 + 2 * k);
         o.h[k] = __floats2half2_rn((v[i][2 * k] - mean) * rstd * gm.x + bt.x, (v[i][2 * k + 1] - mean) * rstd * gm.y + bt.y);
       }
-      *reinterpret_cast<Half8*>(y + m * C + c0) = o;
+      if constexpr (OUT8) *reinterpret_cast<uint2*>(reinterpret_cast<uint8_t*>(y) + m * C + c0) = half8_to_e4m3(o);
+      else *reinterpret_cast<Half8*>(y + m * C + c0) = o;
     }
   }
 }
 
 // generic fallback: one warp per row, up to 10 vectors per lane with masking (any C % 8 == 0, C <= 2560)
-template <int VPL>
+template <int VPL, bool OUT8>
 __global__ void __launch_bounds__(256)
 layernorm_generic_kernel(const __half* __restrict__ x, const __half* __restrict__ addvec, int add_div, int add_mod,
                          long long M, int C, const float* __restrict__ gamma, const float* __restrict__ beta, float eps,
@@ -265,7 +273,8 @@ layernorm_generic_kernel(const __half* __restrict__ x, const __half* __restrict_
         o.h[k] = __floats2half2_rn((v[i][2 * k] - mean) * rstd * gamma[c] + beta[c],
                                    (v[i][2 * k + 1] - mean) * rstd * gamma[c + 1] + beta[c + 1]);
       }
-      *reinterpret_cast<Half8*>(y + m * C + cv * 8) = o;
+      if constexpr (OUT8) *reinterpret_cast<uint2*>(reinterpret_cast<uint8_t*>(y) + m * C + cv * 8) = half8_to_e4m3(o);
+      else *reinterpret_cast<Half8*>(y + m * C + cv * 8) = o;
     }
   }
 }
@@ -293,7 +302,7 @@ static int gn_apply_launch(const char* who, const void* x1, int C1, const void* 
                            int64_t rows_per_sample, const float* sums, const float* stats1, const float* stats2, int unit, int ips,
                            int64_t count_rows, const float* gamma, const float* beta, float eps, int apply_silu, void* y,
                            int64_t y_sample_rows, int64_t y_row_off, void* y_prev_rank, void* y_next_rank, int64_t frame_rows,
-                           void* stream) {
+                           void* stream, bool out8 = false) {
   int rc = gn_check(x1, C1, x2, C2, n_samples, rows_per_sample, who);
   if (rc) return rc;
   if ((y_prev_rank || y_next_rank || frame_rows > 0) &&
@@ -325,13 +334,18 @@ static int gn_apply_launch(const char* who, const void* x1, int C1, const void* 
   slabs = (rows_per_sample + rows_per_cta - 1) / rows_per_cta;
   if (slabs > 2147483647LL) { set_error("%s: too many slabs", who); return -2; }
   if (frame_rows > 0)
-    gn_apply_kernel<true><<<dim3((unsigned)slabs, n_samples), threads, 0, st>>>(
+    gn_apply_kernel<true, false><<<dim3((unsigned)slabs, n_samples), threads, 0, st>>>(
         (const __half*)x1, C1, (const __half*)x2, C2, rows_per_sample, rows_per_cta, sums,
         (double)count_rows * (double)(C / GN_GROUPS), eps, gamma, beta, apply_silu, (__half*)y, y_sample_rows, y_row_off,
         (__half*)y_prev_rank, (__half*)y_next_rank, frame_rows, !y_prev_rank ? 1 : 0, !y_next_rank ? 1 : 0, stats1, stats2,
         unit, ips);
+  else if (out8)
+    gn_apply_kernel<false, true><<<dim3((unsigned)slabs, n_samples), threads, 0, st>>>(
+        (const __half*)x1, C1, (const __half*)x2, C2, rows_per_sample, rows_per_cta, sums,
+        (double)count_rows * (double)(C / GN_GROUPS), eps, gamma, beta, apply_silu, (__half*)y, y_sample_rows, y_row_off,
+        nullptr, nullptr, 0, 0, 0, stats1, stats2, unit, ips);
   else
-    gn_apply_kernel<false><<<dim3((unsigned)slabs, n_samples), threads, 0, st>>>(
+    gn_apply_kernel<false, false><<<dim3((unsigned)slabs, n_samples), threads, 0, st>>>(
         (const __half*)x1, C1, (const __half*)x2, C2, rows_per_sample, rows_per_cta, sums,
         (double)count_rows * (double)(C / GN_GROUPS), eps, gamma, beta, apply_silu, (__half*)y, y_sample_rows, y_row_off,
         nullptr, nullptr, 0, 0, 0, stats1, stats2, unit, ips);
@@ -559,12 +573,29 @@ extern "C" int hi3d_groupnorm_apply_stats(const void* x1, int C1, const float* s
                          y_next_rank, frame_rows, stream);
 }
 
-extern "C" int hi3d_layernorm(const void* x, const void* addvec, int add_div, int add_mod, int64_t M, int C,
-                              const float* gamma, const float* beta, float eps, void* y, void* stream) {
+extern "C" int hi3d_groupnorm_apply_stats_fp8(const void* x1, int C1, const float* stats1, const void* x2, int C2,
+                                              const float* stats2, int unit, int n_samples, int64_t rows_per_sample,
+                                              int imgs_per_sample, int64_t count_rows, const float* gamma, const float* beta,
+                                              float eps, int apply_silu, void* y, void* stream) {
+  if (!x2) { C2 = 0; stats2 = nullptr; }
+  if (!stats1 || (x2 && !stats2) || imgs_per_sample <= 0) {
+    set_error("hi3d_groupnorm_apply_stats_fp8: null statistics table");
+    return -2;
+  }
+  int rc = unit_check(C1, C2, unit, "hi3d_groupnorm_apply_stats_fp8");
+  if (rc) return rc;
+  return gn_apply_launch("hi3d_groupnorm_apply_stats_fp8", x1, C1, x2, C2, n_samples, rows_per_sample, nullptr, stats1, stats2,
+                         unit, imgs_per_sample, count_rows, gamma, beta, eps, apply_silu, y, 0, 0, nullptr, nullptr, 0, stream,
+                         true);
+}
+
+// The one launcher of the LayerNorm kernels; out8: e4m3 output.
+static int layernorm_launch(const char* who, const void* x, const void* addvec, int add_div, int add_mod, int64_t M, int C,
+                            const float* gamma, const float* beta, float eps, void* y, void* stream, bool out8) {
   if (!x || !y || !gamma || !beta || M <= 0 || C <= 0 || (C % 8) || C > 2560 || ((uintptr_t)x & 15) ||
       ((uintptr_t)y & 15) || ((uintptr_t)gamma & 7) || ((uintptr_t)beta & 7) ||
       (addvec && (add_div <= 0 || add_mod <= 0 || ((uintptr_t)addvec & 15)))) {
-    set_error("hi3d_layernorm: bad arguments (M=%lld C=%d)", (long long)M, C);
+    set_error("%s: bad arguments (M=%lld C=%d)", who, (long long)M, C);
     return -2;
   }
   cudaStream_t st = (cudaStream_t)stream;
@@ -576,14 +607,16 @@ extern "C" int hi3d_layernorm(const void* x, const void* addvec, int add_div, in
   do {                                                                                                                  \
     const long long rows_per_cta = 8 * (32 / LPR);                                                                      \
     const long long blocks = (M + rows_per_cta - 1) / rows_per_cta;                                                     \
-    if (blocks > 2147483647LL) { set_error("hi3d_layernorm: M too large"); return -2; }                                 \
-    layernorm_kernel<VPL, LPR><<<(unsigned)blocks, 256, 0, st>>>(xp, ap, add_div, add_mod, M, C, gamma, beta, eps, yp);  \
+    if (blocks > 2147483647LL) { set_error("%s: M too large", who); return -2; }                                 \
+    if (out8) layernorm_kernel<VPL, LPR, true><<<(unsigned)blocks, 256, 0, st>>>(xp, ap, add_div, add_mod, M, C, gamma, beta, eps, yp); \
+    else layernorm_kernel<VPL, LPR, false><<<(unsigned)blocks, 256, 0, st>>>(xp, ap, add_div, add_mod, M, C, gamma, beta, eps, yp); \
   } while (0)
 #define HI3D_LN_GENERIC(VPL)                                                                                             \
   do {                                                                                                                  \
     const long long blocks = (M + 7) / 8;                                                                               \
-    if (blocks > 2147483647LL) { set_error("hi3d_layernorm: M too large"); return -2; }                                 \
-    layernorm_generic_kernel<VPL><<<(unsigned)blocks, 256, 0, st>>>(xp, ap, add_div, add_mod, M, C, gamma, beta, eps, yp); \
+    if (blocks > 2147483647LL) { set_error("%s: M too large", who); return -2; }                                 \
+    if (out8) layernorm_generic_kernel<VPL, true><<<(unsigned)blocks, 256, 0, st>>>(xp, ap, add_div, add_mod, M, C, gamma, beta, eps, yp); \
+    else layernorm_generic_kernel<VPL, false><<<(unsigned)blocks, 256, 0, st>>>(xp, ap, add_div, add_mod, M, C, gamma, beta, eps, yp); \
   } while (0)
   if (CV == 40) HI3D_LN_LAUNCH(5, 8);            // C = 320
   else if (CV == 80) HI3D_LN_LAUNCH(5, 16);      // C = 640
@@ -598,5 +631,16 @@ extern "C" int hi3d_layernorm(const void* x, const void* addvec, int add_div, in
   else HI3D_LN_GENERIC(10);
 #undef HI3D_LN_LAUNCH
 #undef HI3D_LN_GENERIC
-  return check_launch("hi3d_layernorm");
+  return check_launch(who);
+}
+
+
+extern "C" int hi3d_layernorm(const void* x, const void* addvec, int add_div, int add_mod, int64_t M, int C,
+                              const float* gamma, const float* beta, float eps, void* y, void* stream) {
+  return layernorm_launch("hi3d_layernorm", x, addvec, add_div, add_mod, M, C, gamma, beta, eps, y, stream, false);
+}
+
+extern "C" int hi3d_layernorm_fp8(const void* x, const void* addvec, int add_div, int add_mod, int64_t M, int C,
+                                  const float* gamma, const float* beta, float eps, void* y, void* stream) {
+  return layernorm_launch("hi3d_layernorm_fp8", x, addvec, add_div, add_mod, M, C, gamma, beta, eps, y, stream, true);
 }

@@ -16,6 +16,7 @@ from ._native import (ACT_GEGLU, ACT_GELU, ACT_NONE, ACT_QUICKGELU, ACT_RELU, AC
                       ROWS_TEMPORAL)
 
 F16 = torch.float16
+E4M3 = torch.float8_e4m3fn
 
 
 def _stream() -> int:
@@ -32,6 +33,17 @@ def _chk16(t: torch.Tensor, name: str):
                          f"contiguous={t.is_contiguous()}")
 
 
+def _chk8(t: torch.Tensor, name: str):
+    if t.dtype != E4M3 or not t.is_cuda or not t.is_contiguous():
+        raise ValueError(f"{name}: expected a contiguous CUDA float8_e4m3fn tensor, got {t.dtype} {t.device} "
+                         f"contiguous={t.is_contiguous()}")
+
+
+def _chk_act(t: torch.Tensor, name: str):
+    """fp16 or e4m3 activation tensor (a GEMM operand or a normalisation output)"""
+    (_chk8 if t.dtype == E4M3 else _chk16)(t, name)
+
+
 def _chk32(t: torch.Tensor, name: str):
     if t.dtype != torch.float32 or not t.is_cuda or not t.is_contiguous():
         raise ValueError(f"{name}: expected a contiguous CUDA fp32 tensor")
@@ -43,7 +55,7 @@ class SegSpec:
 
     def __init__(self, src: torch.Tensor, C_: Optional[int] = None, c_off: int = 0, dy: int = 0, dx: int = 0,
                  dt: int = 0, ld: Optional[int] = None):
-        _chk16(src, "segment source")
+        _chk_act(src, "segment source")
         self.src = src
         self.ld = src.shape[-1] if ld is None else ld
         self.C = (self.ld - c_off) if C_ is None else C_
@@ -71,15 +83,39 @@ def temporal_taps(src: torch.Tensor) -> List[SegSpec]:
     return [SegSpec(src, dt=d) for d in (-1, 0, 1)]
 
 
+def fp8_covers(mode: int, M: int, Nn: int, geom: Optional[dict] = None) -> bool:
+    """Whether hi3d_gemm_tc5_fp8 covers a one-source GEMM of this geometry (hi3d_gemm_tc5_fp8_covers, the engine's own tiling
+    rules): the e4m3 engine has no fallback, so a plan runs a shape it does not cover in fp16."""
+    g = geom or {}
+    p = N.GemmParams()
+    p.M, p.N, p.K, p.mode = M, Nn, 64, mode
+    p.Ho, p.Wo = g.get("Ho", 1), g.get("Wo", 1)
+    p.Hs, p.Ws = g.get("Hs", p.Ho), g.get("Ws", p.Wo)
+    p.stride, p.ups, p.T = g.get("stride", 1), g.get("ups", 0), g.get("T", 1)
+    p.nseg = 1
+    p.seg[0].C = 64
+    rc = N.load().hi3d_gemm_tc5_fp8_covers(C.byref(p))
+    if rc < 0:
+        N.check(rc, "hi3d_gemm_tc5_fp8_covers")
+    return rc == 1
+
+
 class Gemm:
-    """out[M, N(/2)] = epilogue(A_gather[M, K] @ W[N, K]^T): one pre-baked hi3d_gemm_params block."""
+    """out[M, N(/2)] = epilogue(A_gather[M, K] @ W[N, K]^T): one pre-baked hi3d_gemm_params block.
+
+    e4m3 W (pack.pack_e4m3): every segment source is e4m3 too, `w_scale` is W's fp32 [N] scale and the call runs
+    hi3d_gemm_tc5_fp8 whatever the engine; `out` may then be fp16 or e4m3."""
 
     def __init__(self, segs: Sequence[SegSpec], W: torch.Tensor, out: torch.Tensor, M: int, *, mode: int = ROWS_PLAIN,
                  geom: Optional[dict] = None, bias: Optional[torch.Tensor] = None,
                  rowbias: Optional[torch.Tensor] = None, rb_div: int = 1, rb_mod: int = 1, act: int = ACT_NONE,
                  residual: Optional[torch.Tensor] = None, blend_x: Optional[torch.Tensor] = None, alpha: float = 0.0,
-                 engine: str = "mma"):
-        if out.is_contiguous():
+                 engine: str = "mma", w_scale: Optional[torch.Tensor] = None):
+        out_fp8 = out.dtype == E4M3
+        if out_fp8:
+            _chk8(out, "out")
+            out_ld, out_rows = out.shape[-1], out.numel() // out.shape[-1]
+        elif out.is_contiguous():
             _chk16(out, "out")
             out_ld, out_rows = out.shape[-1], out.numel() // out.shape[-1]
         else:                       # a column slice of a wider matrix (a channel slice of a concat buffer): rows of stride out_ld
@@ -87,7 +123,22 @@ class Gemm:
                 raise ValueError(f"out: expected a contiguous CUDA fp16 tensor or a column slice of one, got {out.dtype} "
                                  f"{out.device} {tuple(out.shape)} strides {out.stride()}")
             out_ld, out_rows = out.stride(0), out.shape[0]
-        _chk16(W, "W")
+        fp8 = W.dtype == E4M3
+        if fp8:
+            _chk8(W, "W")
+            if w_scale is None:
+                raise ValueError("an e4m3 W needs its w_scale")
+            _chk32(w_scale, "w_scale")
+            if w_scale.numel() != W.shape[0]:
+                raise ValueError(f"w_scale has {w_scale.numel()} entries for N = {W.shape[0]}")
+            if any(s.src.dtype != E4M3 for s in segs):
+                raise ValueError("an e4m3 W needs e4m3 segment sources")
+        else:
+            _chk16(W, "W")
+            if w_scale is not None or any(s.src.dtype != F16 for s in segs):
+                raise ValueError("an fp16 W takes fp16 segment sources and no w_scale")
+            if out_fp8:
+                raise ValueError("an e4m3 output needs e4m3 operands")
         Nn, K = W.shape
         if len(segs) > N.MAX_SEGS:
             raise ValueError(f"too many segments ({len(segs)})")
@@ -129,15 +180,20 @@ class Gemm:
         if out.shape[-1] < n_out or out_rows < M * (4 if p.out_up else 1):
             raise ValueError(f"out too small: {tuple(out.shape)} for M={M} N_out={n_out}")
         self.p = p
-        self._keep = (list(segs), W, out, bias, rowbias, residual, blend_x)   # keep storages alive
-        self._fn = N.load().hi3d_gemm_tc5 if engine == "tc5" else N.load().hi3d_gemm
+        self._keep = (list(segs), W, out, bias, rowbias, residual, blend_x, w_scale)   # keep storages alive
+        if fp8:
+            fn8, ws, o8 = N.load().hi3d_gemm_tc5_fp8, w_scale.data_ptr(), int(out_fp8)
+            self._fn = lambda pp, st: fn8(pp, ws, o8, st)
+        else:
+            self._fn = N.load().hi3d_gemm_tc5 if engine == "tc5" else N.load().hi3d_gemm
+        self.fp8 = fp8
         self.flops = 2.0 * M * Nn * K
         self.out = out
 
     def __call__(self):
         rc = self._fn(C.byref(self.p), _stream())
         if rc:
-            N.check(rc, "hi3d_gemm")
+            N.check(rc, "hi3d_gemm_tc5_fp8" if self.fp8 else "hi3d_gemm")
 
 
 # ------------------------------------------------------------------------------------------------------
@@ -160,11 +216,22 @@ def groupnorm_apply_stats(x1: torch.Tensor, stats1: torch.Tensor, x2: Optional[t
                           gamma: torch.Tensor, beta: torch.Tensor, eps: float, silu: bool, y: torch.Tensor,
                           y_sample_rows: int = 0, y_row_off: int = 0, y_prev: Optional[int] = None, y_next: Optional[int] = None,
                           frame_rows: int = 0):
-    """GroupNorm(32)[+SiLU] in ONE launch: statistics from the unit tables of x1 / x2 (groupnorm_unit_stats)."""
-    _chk16(x1, "x1"); _chk16(y, "y"); _chk32(stats1, "stats1"); _chk32(gamma, "gamma"); _chk32(beta, "beta")
+    """GroupNorm(32)[+SiLU] in ONE launch: statistics from the unit tables of x1 / x2 (groupnorm_unit_stats).
+    An e4m3 y (dense, no halo arguments) selects hi3d_groupnorm_apply_stats_fp8."""
+    _chk16(x1, "x1"); _chk_act(y, "y"); _chk32(stats1, "stats1"); _chk32(gamma, "gamma"); _chk32(beta, "beta")
     c2 = 0 if x2 is None else x2.shape[-1]
     if x2 is not None:
         _chk16(x2, "x2"); _chk32(stats2, "stats2")
+    if y.dtype == E4M3:
+        if y_sample_rows or y_row_off or y_prev is not None or y_next is not None or frame_rows:
+            raise ValueError("groupnorm_apply_stats: an e4m3 output is dense (no halo arguments)")
+        if y.numel() < n_samples * rows_per_sample * (x1.shape[-1] + c2):
+            raise ValueError(f"groupnorm_apply_stats: y {tuple(y.shape)} too small")
+        N.check(N.load().hi3d_groupnorm_apply_stats_fp8(x1.data_ptr(), x1.shape[-1], stats1.data_ptr(), _ptr(x2), c2, _ptr(stats2),
+                                                        unit, n_samples, rows_per_sample, imgs_per_sample, count_rows,
+                                                        gamma.data_ptr(), beta.data_ptr(), eps, int(silu), y.data_ptr(), _stream()),
+                "hi3d_groupnorm_apply_stats_fp8")
+        return
     N.check(N.load().hi3d_groupnorm_apply_stats(x1.data_ptr(), x1.shape[-1], stats1.data_ptr(), _ptr(x2), c2, _ptr(stats2), unit,
                                                 n_samples, rows_per_sample, imgs_per_sample, count_rows, gamma.data_ptr(),
                                                 beta.data_ptr(), eps, int(silu), y.data_ptr(), y_sample_rows, y_row_off, y_prev,
@@ -186,11 +253,15 @@ def groupnorm_group_sums(stats1: torch.Tensor, C1: int, stats2: Optional[torch.T
 
 def layernorm(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, y: torch.Tensor, M: int,
               addvec: Optional[torch.Tensor] = None, add_div: int = 1, add_mod: int = 1, eps: float = 1e-5):
-    _chk16(x, "x"); _chk16(y, "y"); _chk32(gamma, "gamma"); _chk32(beta, "beta")
+    """An e4m3 y selects hi3d_layernorm_fp8."""
+    _chk16(x, "x"); _chk_act(y, "y"); _chk32(gamma, "gamma"); _chk32(beta, "beta")
     if addvec is not None:
         _chk16(addvec, "addvec")
-    N.check(N.load().hi3d_layernorm(x.data_ptr(), _ptr(addvec), add_div, add_mod, M, x.shape[-1], gamma.data_ptr(),
-                                    beta.data_ptr(), eps, y.data_ptr(), _stream()), "hi3d_layernorm")
+    if y.dtype == E4M3 and (y.shape[-1] != x.shape[-1] or y.numel() < M * x.shape[-1]):
+        raise ValueError(f"layernorm: e4m3 y {tuple(y.shape)} does not fit [{M}, {x.shape[-1]}]")
+    fn = N.load().hi3d_layernorm_fp8 if y.dtype == E4M3 else N.load().hi3d_layernorm
+    N.check(fn(x.data_ptr(), _ptr(addvec), add_div, add_mod, M, x.shape[-1], gamma.data_ptr(), beta.data_ptr(), eps, y.data_ptr(),
+               _stream()), "hi3d_layernorm_fp8" if y.dtype == E4M3 else "hi3d_layernorm")
 
 
 def attention_d64(qkv: torch.Tensor, n_img: int, L: int, heads: int, out: torch.Tensor, scale: float = 0.125,

@@ -7,6 +7,8 @@ from typing import Optional, Tuple
 import torch
 
 F16 = torch.float16
+E4M3 = torch.float8_e4m3fn
+E4M3_MAX = 448.0
 
 
 def _pad_to(x: int, m: int) -> int:
@@ -88,3 +90,16 @@ def pack_upconv_parity(w: torch.Tensor):
 def cat_k(*mats: torch.Tensor) -> torch.Tensor:
     """Concatenate packed matrices along K (e.g. [3x3 conv | 1x1 skip] fused into one GEMM)."""
     return torch.cat(mats, dim=1).contiguous()
+
+
+def pack_e4m3(w: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Packed fp16 [N, K] weight matrix -> (e4m3 [N, K], fp32 [N] scale) for hi3d_gemm_tc5_fp8: row n is stored as
+    w[n] / scale[n] rounded to nearest even and saturated to +-448, with scale[n] = amax(|w[n]|) / 448 (1 for an all-zero row),
+    so that w[n] ~ e4m3[n] * scale[n].  Zero padding along K stays zero."""
+    if w.dtype != F16 or w.dim() != 2:
+        raise ValueError(f"pack_e4m3: expected a packed fp16 [N, K] matrix, got {w.dtype} {tuple(w.shape)}")
+    wf = w.float()
+    amax = wf.abs().amax(dim=1)
+    scale = torch.where(amax > 0, amax / E4M3_MAX, torch.ones_like(amax))
+    q = (wf / scale[:, None]).clamp(-E4M3_MAX, E4M3_MAX).to(E4M3)
+    return q.contiguous(), scale.contiguous()

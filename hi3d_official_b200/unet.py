@@ -29,6 +29,8 @@ from . import ops, pack
 from .spec import Layer, UNetConfig, unet_param_shapes, unet_plan
 
 F16 = torch.float16
+E4M3 = torch.float8_e4m3fn
+PRECISIONS = ("fp16", "fp8")
 CIN_PAD = 64     # UNet input channels are zero-padded to one 64-wide K segment per tap
 COUT_PAD = 8     # final conv output channels padded to the engine's N granularity
 
@@ -54,12 +56,15 @@ class Arena:
     def __init__(self, device, peer_group=None, symm_tags=()):
         self.device = device
         self.req: Dict[str, int] = {}
+        self.dtypes: Dict[str, torch.dtype] = {}      # element type per tag: fp16, or e4m3 for the operands of FP8 GEMMs
         self.bufs: Dict[str, torch.Tensor] = {}
         self.views: List[Tuple[str, int, int, list]] = []
         self.peer_group, self.symm_tags = peer_group, tuple(symm_tags)
         self.symm: Dict[str, object] = {}
 
-    def want(self, tag: str, rows: int, cols: int) -> "LazyBuf":
+    def want(self, tag: str, rows: int, cols: int, dtype: torch.dtype = F16) -> "LazyBuf":
+        if self.dtypes.setdefault(tag, dtype) != dtype or (dtype != F16 and tag in self.symm_tags):
+            raise ValueError(f"arena tag {tag!r} requested as {dtype} and as {self.dtypes[tag]}")
         n = rows * cols
         self.req[tag] = max(self.req.get(tag, 0), n)
         return LazyBuf(self, tag, rows, cols)
@@ -72,7 +77,7 @@ class Arena:
                     self.symm[tag] = sb
                     self.bufs[tag] = sb.view(F16)[:n]
                 else:
-                    self.bufs[tag] = torch.zeros(n, dtype=F16, device=self.device)
+                    self.bufs[tag] = torch.zeros(n, dtype=self.dtypes[tag], device=self.device)
 
     def peers(self, tag: str):
         """peer.SymmBuffer of a symmetric tag (views of a tag start at offset 0, so the peers' base pointers address the same
@@ -83,7 +88,7 @@ class Arena:
         return self.bufs[tag][: rows * cols].view(rows, cols)
 
     def nbytes(self) -> int:
-        return sum(b.numel() * 2 for b in self.bufs.values())
+        return sum(b.numel() * b.element_size() for b in self.bufs.values())
 
 
 class LazyBuf:
@@ -149,8 +154,10 @@ class VideoUNet(nn.Module):
         for k, m in tree._modules.items():
             self.add_module(k, m)
         self._packed: Optional[dict] = None
+        self._packed8: Optional[dict] = None
         self._plans: Dict[tuple, "_Plan"] = {}
         self.engine = os.environ.get("HI3D_ENGINE", "tc5")     # "tc5" = TMA + wgmma engine, "mma" = mma.sync engine
+        self.precision = "fp16"
         # packed weights, launch plans and captured graphs derive from the parameters: ANY load that reaches this module
         # -- its own load_state_dict or a parent's (DiffusionEngine.init_from_ckpt recurses through
         # _load_from_state_dict and never calls the override below) -- must drop them
@@ -158,7 +165,7 @@ class VideoUNet(nn.Module):
 
     # ---- parameter lifecycle ---------------------------------------------------------------------------
     def _invalidate(self):
-        self._packed = None
+        self._packed = self._packed8 = None
         self._plans = {}
 
     def _apply(self, fn, *a, **k):
@@ -174,6 +181,18 @@ class VideoUNet(nn.Module):
             raise ValueError(engine)
         if engine != self.engine:
             self.engine = engine
+            self._plans = {}
+
+    def set_precision(self, precision: str):
+        """Operand precision of the UNet's large GEMMs.  "fp16" (default): every GEMM in fp16.  "fp8": the ResBlock convs, the
+        temporal convs, proj_in, the attention q|k|v projections and the feed-forwards take e4m3 operands (per-output-row weight
+        scales, unscaled normalised activations written as e4m3 by their GroupNorm / LayerNorm / GEGLU producers); every other
+        layer stays fp16.  A precision the user chooses, like the sampler: fp8 does not compute what fp16 computes.  Cached
+        plans are dropped, as set_engine does."""
+        if precision not in PRECISIONS:
+            raise ValueError(f"precision {precision!r}: expected one of {PRECISIONS}")
+        if precision != self.precision:
+            self.precision = precision
             self._plans = {}
 
     @property
@@ -258,6 +277,38 @@ class VideoUNet(nn.Module):
         self._packed = P
         return P
 
+    def _pack_fp8(self) -> dict:
+        """e4m3 twins (pack.pack_e4m3: (W, w_scale)) of the packed weights an fp8 plan runs in FP8.  A channel-changing ResBlock's
+        conv2 gets its own weight and bias ("conv2", "conv2.bias") and its 1x1 skip an fp16 one ("skip"): the skip reads the
+        block input, which no norm has scaled to O(1), so fp8 plans run it as its own fp16 GEMM instead of extra K segments."""
+        if self._packed8 is not None:
+            return self._packed8
+        P, Q = self._pack(), {}
+        sd = {k: v.detach() for k, v in self.state_dict().items()}
+        q8 = pack.pack_e4m3
+        for L in [L for blk in self.plan_desc.input_blocks + [self.plan_desc.middle] + self.plan_desc.output_blocks for L in blk]:
+            n = L.name
+            if L.kind == "res":
+                for q, pk in ((n, pack.pack_conv2d), (n + "time_stack.", pack.pack_conv3d_t)):
+                    Q[q + "conv1"] = q8(P[q + "conv1"][0])
+                    if q + "skip_connection.weight" in sd:
+                        Q[q + "conv2"] = q8(pk(sd[q + "out_layers.3.weight"]))
+                        Q[q + "conv2.bias"] = pack.pack_bias(sd[q + "out_layers.3.bias"], L.cout)
+                        Q[q + "skip"] = (pack.pack_conv2d(sd[q + "skip_connection.weight"]),
+                                         pack.pack_bias(sd[q + "skip_connection.bias"], L.cout))
+                    else:
+                        Q[q + "conv2"] = q8(P[q + "conv2"][0])
+            elif L.kind == "attn":
+                Q[n + "proj_in"] = q8(P[n + "proj_in"][0])
+                for d in range(self.cfg.transformer_depth):
+                    for q, temporal in ((n + f"transformer_blocks.{d}.", False), (n + f"time_stack.{d}.", True)):
+                        Q[q + "qkv"] = q8(P[q + "qkv"])
+                        for ff in ("ff",) + (("ff_in",) if temporal else ()):
+                            Q[q + ff + "1"] = q8(P[q + ff + "1"][0])
+                            Q[q + ff + "2"] = q8(P[q + ff + "2"][0])
+        self._packed8 = Q
+        return Q
+
     # ---- plans --------------------------------------------------------------------------------------------
     def get_plan(self, N: int, H: int, W: int, T: int, shard: Optional[Tuple[int, int]] = None) -> "_Plan":
         """shard = (rank, world): frame-sharded plan -- N = B * T local samples, this rank owns frames
@@ -297,6 +348,10 @@ class _Plan:
 
     def __init__(self, net: VideoUNet, N: int, H: int, W: int, T: int, shard: Optional[Tuple[int, int]] = None):
         self.shard = None if shard is None or shard[1] == 1 else (int(shard[0]), int(shard[1]))
+        self.fp8 = net.precision == "fp8"
+        if self.fp8 and self.shard:
+            raise NotImplementedError("fp8 precision is not built for frame-sharded plans; use fp16")
+        self.fp8_layers: List[str] = []    # state-dict names of the layers this plan runs with e4m3 operands, in plan order
         self.rank, self.world = self.shard if self.shard else (0, 1)
         self.Tg = T * self.world                     # frames per clip over all ranks
         if N % T:
@@ -384,13 +439,15 @@ class _Plan:
             dist.barrier(group=self.peer.pg)
 
     # ---- helpers -----------------------------------------------------------------------------------------------
-    def _gemm(self, lst, segs_fn, W, out: LazyBuf, M, **kw):
-        """Defer Gemm construction until buffers exist. segs_fn() -> list[SegSpec]; tensor kwargs may be LazyBuf."""
+    def _gemm(self, lst, segs_fn, W, out: LazyBuf, M, layers: Optional[List[str]] = None, **kw):
+        """Defer Gemm construction until buffers exist. segs_fn() -> list[SegSpec]; tensor kwargs may be LazyBuf.  layers: the
+        state-dict layers the GEMM computes (kept as Gemm.layers, for tests that check a layer against the reference)."""
         def build():
             k2 = {}
             for k, v in kw.items():
                 k2[k] = v.t if isinstance(v, LazyBuf) else v
             g = ops.Gemm(segs_fn(), W, out.t if isinstance(out, LazyBuf) else out, M, engine=self.engine, **k2)
+            g.layers = layers
             self.flops += g.flops if lst is self._build else 0.0
             return g
         lst.append(build)
@@ -405,6 +462,25 @@ class _Plan:
                 torch.cuda.nvtx.range_push(name)
                 self._nvtx_open = True
             self._call(self._build, m, kind="marker")
+
+    def _fp8_for(self, mode: int, M: int, N: int, geom: Optional[dict] = None) -> bool:
+        """Whether an fp8 plan runs this GEMM in FP8: every layer of the FP8 set whose shape the e4m3 engine covers (all of them
+        at the sampler's latent sizes; the smallest levels of tiny latents stay fp16)."""
+        return self.fp8 and ops.fp8_covers(mode, M, N, geom)
+
+    def _wt(self, key: str, names: List[str], fp8: bool):
+        """(W, kw) of packed layer `key`, the state-dict layers `names`: fp16 W, or with fp8 its e4m3 twin, recording `names`
+        in fp8_layers.  kw = the Gemm keywords that go with W: w_scale (None for fp16) and layers."""
+        if not fp8:
+            w = self.P[key]
+            return (w[0] if isinstance(w, tuple) else w), dict(w_scale=None, layers=names)
+        self.fp8_layers += names
+        W8, ws = self.net._pack_fp8()[key]
+        return W8, dict(w_scale=ws, layers=names)
+
+    def _act(self, tag: str, rows: int, cols: int, fp8: bool) -> LazyBuf:
+        """Arena buffer of a normalised GEMM operand: fp16, or with fp8 e4m3 (tag + "8")."""
+        return self.arena.want(tag + "8", rows, cols, E4M3) if fp8 else self.arena.want(tag, rows, cols)
 
     def _stats(self, n_img: int, C: int) -> StatsBuf:
         sb = StatsBuf(self, self._stats_floats, n_img, C // self.gn_unit)
@@ -558,19 +634,33 @@ class _Plan:
         cin, cout = sum(cs), L.cout
         x1 = srcs[0][0]
         x2 = srcs[1][0] if len(srcs) > 1 else None
-        g_in = A.want("gn", M, cin)
+        conv8 = self._fp8_for(ops.ROWS_CONV2D, M, cout, dict(Ho=h, Wo=w))
+        temp8 = self.shard is None and self._fp8_for(ops.ROWS_TEMPORAL, M, cout, dict(Ho=HW, Wo=1, T=T))
+        g_in = self._act("gn", M, cin, conv8)
         hbuf = A.want("h", M, cout)
-        g_mid = A.want("gn", M, cout)
+        g_mid = self._act("gn", M, cout, conv8)
         xs = A.want("xs", M, cout)
         st_h1, st_xs, st_h2 = self._stats(N, cout), self._stats(N, cout), self._stats(N, cout)
         # -- spatial half
         emit_groupnorm(bl, [(s_[0], s_[4]) for s_ in srcs], unit, N, HW, 1, P[n + "gn1"], 1e-5, True, g_in)
         emb1 = self._emb_slice(n)
-        self._gemm(bl, lambda: ops.conv_taps([g_in.t]), P[n + "conv1"][0], hbuf, M, mode=ops.ROWS_CONV2D,
-                   geom=dict(Ho=h, Wo=w, Hs=h, Ws=w), bias=P[n + "conv1"][1], rowbias=emb1, rb_div=HW, rb_mod=N)
+        W1, kw1 = self._wt(n + "conv1", [n + "in_layers.2"], conv8)
+        self._gemm(bl, lambda: ops.conv_taps([g_in.t]), W1, hbuf, M, mode=ops.ROWS_CONV2D,
+                   geom=dict(Ho=h, Wo=w, Hs=h, Ws=w), bias=P[n + "conv1"][1], rowbias=emb1, rb_div=HW, rb_mod=N, **kw1)
         emit_unit_stats(bl, hbuf, st_h1, unit)
         emit_groupnorm(bl, [(hbuf, st_h1)], unit, N, HW, 1, P[n + "gn2"], 1e-5, True, g_mid)
-        if cin != cout:
+        if conv8:
+            # the 1x1 skip (fp16, over the un-normalised block input) becomes conv2's residual
+            W2, kw2 = self._wt(n + "conv2", [n + "out_layers.3"], True)
+            res, b2 = x1, P[n + "conv2"][1]
+            if cin != cout:
+                Q = self.net._pack_fp8()
+                res, b2 = A.want("skip", M, cout), Q[n + "conv2.bias"]
+                self._gemm(bl, lambda: [ops.SegSpec(s_[0].t) for s_ in srcs], Q[n + "skip"][0], res, M, bias=Q[n + "skip"][1],
+                           layers=[n + "skip_connection"])
+            self._gemm(bl, lambda: ops.conv_taps([g_mid.t]), W2, xs, M, mode=ops.ROWS_CONV2D, geom=dict(Ho=h, Wo=w, Hs=h, Ws=w),
+                       bias=b2, residual=res, **kw2)
+        elif cin != cout:
             self._gemm(bl, lambda: ops.conv_taps([g_mid.t]) + [ops.SegSpec(s_[0].t) for s_ in srcs], P[n + "conv2"][0], xs, M,
                        mode=ops.ROWS_CONV2D, geom=dict(Ho=h, Wo=w, Hs=h, Ws=w), bias=P[n + "conv2"][1])
         else:
@@ -584,15 +674,18 @@ class _Plan:
         g4, b4 = P[q + "gn2"]
         emb2 = self._emb_slice(q)
         if self.shard is None:
-            emit_groupnorm(bl, [(xs, st_xs)], unit, B, T * HW, T, (g3, b3), 1e-5, True, g_mid)
+            g_t = self._act("gn", M, cout, temp8)
+            emit_groupnorm(bl, [(xs, st_xs)], unit, B, T * HW, T, (g3, b3), 1e-5, True, g_t)
             geo = dict(Ho=HW, Wo=1, T=T)
-            self._gemm(bl, lambda: ops.temporal_taps(g_mid.t), P[q + "conv1"][0], hbuf, M, mode=ops.ROWS_TEMPORAL, geom=geo,
-                       bias=P[q + "conv1"][1], rowbias=emb2, rb_div=HW, rb_mod=N)
+            W3, kw3 = self._wt(q + "conv1", [q + "in_layers.2"], temp8)
+            self._gemm(bl, lambda: ops.temporal_taps(g_t.t), W3, hbuf, M, mode=ops.ROWS_TEMPORAL, geom=geo,
+                       bias=P[q + "conv1"][1], rowbias=emb2, rb_div=HW, rb_mod=N, **kw3)
             emit_unit_stats(bl, hbuf, st_h2, unit)
-            emit_groupnorm(bl, [(hbuf, st_h2)], unit, B, T * HW, T, (g4, b4), 1e-5, True, g_mid)
+            emit_groupnorm(bl, [(hbuf, st_h2)], unit, B, T * HW, T, (g4, b4), 1e-5, True, g_t)
             # x_t = xs + conv(...);  out = alpha*xs + (1-alpha)*x_t   (util.py:358-369)
-            self._gemm(bl, lambda: ops.temporal_taps(g_mid.t), P[q + "conv2"][0], out, M, mode=ops.ROWS_TEMPORAL, geom=geo,
-                       bias=P[q + "conv2"][1], residual=xs, blend_x=xs, alpha=P[n + "alpha"])
+            W4, kw4 = self._wt(q + "conv2", [q + "out_layers.3"], temp8)
+            self._gemm(bl, lambda: ops.temporal_taps(g_t.t), W4, out, M, mode=ops.ROWS_TEMPORAL, geom=geo,
+                       bias=P[q + "conv2"][1], residual=xs, blend_x=xs, alpha=P[n + "alpha"], **kw4)
             emit_unit_stats(bl, out, out_stats, unit)
             return
         # frames sharded over ranks (SURVEY F9 / 8e): the (T,H,W) statistics need the (sum, sumsq) of every rank, the GN
@@ -649,8 +742,10 @@ class _Plan:
         if self.net.cfg.num_head_channels != 64:
             raise NotImplementedError("attention kernels are specialised for head dim 64")
         dev = self.dev
-        gn, t0, t1, t2 = A.want("gn", M, C), A.want("t0", M, C), A.want("t1", M, C), A.want("t2", M, C)
-        ln, qkv, att, ffh = A.want("ln", M, C), A.want("qkv", M, 3 * C), A.want("att", M, C), A.want("ffh", M, 4 * C)
+        f8 = self._fp8_for(ops.ROWS_PLAIN, M, C)
+        gn, t0, t1, t2 = self._act("gn", M, C, f8), A.want("t0", M, C), A.want("t1", M, C), A.want("t2", M, C)
+        ln, qkv, att = self._act("ln", M, C, f8), A.want("qkv", M, 3 * C), A.want("att", M, C)
+        ffh = self._act("ffh", M, 4 * C, f8)
         # time_pos_embed(timestep_embedding(arange(T))) : plan constant (video_attention.py:266-276)
         tpe_in = torch.zeros(T, C, dtype=F16, device=dev)
         tpe_h = torch.zeros(T, 4 * C, dtype=F16, device=dev)
@@ -660,7 +755,8 @@ class _Plan:
         ops.Gemm([ops.SegSpec(tpe_h)], P[n + "tpe2"][0], emb_t, T, bias=P[n + "tpe2"][1])()
 
         emit_groupnorm(bl, [(x, xin[4])], self.gn_unit, N, HW, 1, P[n + "norm"], 1e-6, False, gn)
-        self._gemm(bl, lambda: [ops.SegSpec(gn.t)], P[n + "proj_in"][0], t0, M, bias=P[n + "proj_in"][1])
+        Wp, kwp = self._wt(n + "proj_in", [n + "proj_in"], f8)
+        self._gemm(bl, lambda: [ops.SegSpec(gn.t)], Wp, t0, M, bias=P[n + "proj_in"][1], **kwp)
         tok = t0
         for d in range(self.net.cfg.transformer_depth):
             qs, qt = n + f"transformer_blocks.{d}.", n + f"time_stack.{d}."
@@ -673,24 +769,29 @@ class _Plan:
             self._gemm(cl, lambda v_t=v_t: [ops.SegSpec(v_t)], P[qt + "ca_out"][0], r_t, B, bias=P[qt + "ca_out"][1])
             # ---- spatial BasicTransformerBlock (attention.py:551-572)
             self._ln(bl, tok, P[qs + "norm1"], ln, M)
-            self._gemm(bl, lambda: [ops.SegSpec(ln.t)], P[qs + "qkv"], qkv, M)
+            Wq, kwq = self._qkv(qs, f8)
+            self._gemm(bl, lambda: [ops.SegSpec(ln.t)], Wq, qkv, M, **kwq)
             self._call(bl, lambda: ops.attention_d64(qkv.t, N, HW, heads, att.t, engine=self.attn_engine), kind="spatial_attention",
                        flops=4.0 * N * HW * HW * C, bytes=8.0 * M * C)
             self.flops += 4.0 * N * HW * HW * C
             self._gemm(bl, lambda: [ops.SegSpec(att.t)], P[qs + "to_out"][0], t1, M, bias=P[qs + "to_out"][1],
                        residual=tok, rowbias=r_s, rb_div=HW, rb_mod=N)
             self._ln(bl, t1, P[qs + "norm3"], ln, M)
-            self._gemm(bl, lambda: [ops.SegSpec(ln.t)], P[qs + "ff1"][0], ffh, M, bias=P[qs + "ff1"][1], act=ops.ACT_GEGLU)
-            self._gemm(bl, lambda: [ops.SegSpec(ffh.t)], P[qs + "ff2"][0], t2, M, bias=P[qs + "ff2"][1], residual=t1)
+            Wf1, kwf1 = self._wt(qs + "ff1", [qs + "ff.net.0.proj"], f8)
+            self._gemm(bl, lambda: [ops.SegSpec(ln.t)], Wf1, ffh, M, bias=P[qs + "ff1"][1], act=ops.ACT_GEGLU, **kwf1)
+            Wf2, kwf2 = self._wt(qs + "ff2", [qs + "ff.net.2"], f8)
+            self._gemm(bl, lambda: [ops.SegSpec(ffh.t)], Wf2, t2, M, bias=P[qs + "ff2"][1], residual=t1, **kwf2)
             # ---- temporal VideoTransformerBlock on x_mix = t2 + emb_t (video_attention.py:109-140, :286-289)
             self._ln(bl, t2, P[qt + "norm_in"], ln, M, addvec=emb_t, add_div=HW, add_mod=T)
-            self._gemm(bl, lambda: [ops.SegSpec(ln.t)], P[qt + "ff_in1"][0], ffh, M, bias=P[qt + "ff_in1"][1],
-                       act=ops.ACT_GEGLU)
+            Wi1, kwi1 = self._wt(qt + "ff_in1", [qt + "ff_in.net.0.proj"], f8)
+            self._gemm(bl, lambda: [ops.SegSpec(ln.t)], Wi1, ffh, M, bias=P[qt + "ff_in1"][1], act=ops.ACT_GEGLU, **kwi1)
             u0 = t0          # the block input `tok` is dead once attn1's output projection has consumed it
-            self._gemm(bl, lambda: [ops.SegSpec(ffh.t)], P[qt + "ff_in2"][0], u0, M, bias=P[qt + "ff_in2"][1],
-                       residual=t2, rowbias=emb_t, rb_div=HW, rb_mod=T)
+            Wi2, kwi2 = self._wt(qt + "ff_in2", [qt + "ff_in.net.2"], f8)
+            self._gemm(bl, lambda: [ops.SegSpec(ffh.t)], Wi2, u0, M, bias=P[qt + "ff_in2"][1],
+                       residual=t2, rowbias=emb_t, rb_div=HW, rb_mod=T, **kwi2)
             self._ln(bl, u0, P[qt + "norm1"], ln, M)
-            self._gemm(bl, lambda: [ops.SegSpec(ln.t)], P[qt + "qkv"], qkv, M)
+            Wq, kwq = self._qkv(qt, f8)
+            self._gemm(bl, lambda: [ops.SegSpec(ln.t)], Wq, qkv, M, **kwq)
             if self.shard is None:
                 self._call(bl, lambda: ops.temporal_attention_d64(qkv.t, B, T, HW, heads, att.t), kind="temporal_attention",
                            flops=4.0 * N * HW * T * C, bytes=8.0 * M * C)
@@ -720,13 +821,19 @@ class _Plan:
             self._gemm(bl, lambda: [ops.SegSpec(att.t)], P[qt + "to_out"][0], t1, M, bias=P[qt + "to_out"][1],
                        residual=u0, rowbias=r_t, rb_div=T * HW, rb_mod=B)
             self._ln(bl, t1, P[qt + "norm3"], ln, M)
-            self._gemm(bl, lambda: [ops.SegSpec(ln.t)], P[qt + "ff1"][0], ffh, M, bias=P[qt + "ff1"][1], act=ops.ACT_GEGLU)
+            Wt1, kwt1 = self._wt(qt + "ff1", [qt + "ff.net.0.proj"], f8)
+            self._gemm(bl, lambda: [ops.SegSpec(ln.t)], Wt1, ffh, M, bias=P[qt + "ff1"][1], act=ops.ACT_GEGLU, **kwt1)
             # x = alpha * x_spatial + (1 - alpha) * x_mix      (video_attention.py:290-294)
-            self._gemm(bl, lambda: [ops.SegSpec(ffh.t)], P[qt + "ff2"][0], t0, M, bias=P[qt + "ff2"][1], residual=t1,
-                       blend_x=t2, alpha=P[n + "alpha"])
+            Wt2, kwt2 = self._wt(qt + "ff2", [qt + "ff.net.2"], f8)
+            self._gemm(bl, lambda: [ops.SegSpec(ffh.t)], Wt2, t0, M, bias=P[qt + "ff2"][1], residual=t1,
+                       blend_x=t2, alpha=P[n + "alpha"], **kwt2)
             tok = t0
         self._gemm(bl, lambda: [ops.SegSpec(tok.t)], P[n + "proj_out"][0], out, M, bias=P[n + "proj_out"][1], residual=x)
         emit_unit_stats(bl, out, out_stats, self.gn_unit)
+
+    def _qkv(self, q: str, fp8: bool):
+        """(W, kw) of the fused q|k|v projection of attention block `q`."""
+        return self._wt(q + "qkv", [q + "attn1.to_q", q + "attn1.to_k", q + "attn1.to_v"], fp8)
 
     def _ln(self, lst, x: LazyBuf, gb, y: LazyBuf, M, addvec=None, add_div=1, add_mod=1):
         g, b = gb

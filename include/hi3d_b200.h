@@ -107,6 +107,18 @@ int hi3d_gemm_tc5(const hi3d_gemm_params* p, void* stream);
  * 8 = single tiles, 16 = pairs; a forced pair mode takes precedence. */
 int hi3d_gemm_tc5_set_pair_mode(int mode);
 int hi3d_gemm_tc5_set_epilogue_warps(int warps);
+/* The same engine with e4m3 (float8_e4m3fn) operands: every segment source and W are e4m3, K-major like the fp16 ones (src
+ * [rows, ld] with ld a multiple of 16, W [N, K]); wgmma k32 with fp32 accumulators.  The epilogue first scales the accumulator
+ * of column n by w_scale[n] (fp32 [N], W's dequantisation scale, see pack.pack_e4m3), then applies exactly the fp16 sequence:
+ * bias, rowbias, activation, residual, blend (rowbias, residual and blend_x stay fp16).  out_fp8 = 0: out is fp16; 1: out is
+ * e4m3, each value the fp16 result converted with cvt.rn.satfinite (nearest even, saturating to +-448).  Tile width, tile pairs
+ * and the hooks above follow the fp16 rules.  There is no other e4m3 engine: a geometry this one does not cover (see
+ * hi3d_gemm_tc5) returns an error. */
+int hi3d_gemm_tc5_fp8(const hi3d_gemm_params* p, const float* w_scale, int out_fp8, void* stream);
+/* Whether hi3d_gemm_tc5_fp8 covers the GEMM described by p: 1 yes, 0 no, negative for malformed parameters.  Only the
+ * geometry is read (M, N, mode, Ho, Wo, Hs, Ws, stride, ups, out_up, T, the segments' sources and lds, rowbias alignment), so a
+ * launch plan can ask before its buffers exist: leave the pointers NULL and list one segment per distinct source. */
+int hi3d_gemm_tc5_fp8_covers(const hi3d_gemm_params* p);
 
 /* Tiny channel counts (UNet input 8|17 ch, VAE image 3 ch / latent 4 ch) are zero-padded to 64 channels by
  * hi3d_sampler_pre / hi3d_nchw_to_nhwc so that the same engine serves input_blocks.0.0 (video_model.py:186-191),
@@ -143,6 +155,13 @@ int hi3d_groupnorm_apply_stats(const void* x1, int C1, const float* stats1, cons
                                const float* gamma, const float* beta, float eps, int apply_silu, void* y, int64_t y_sample_rows,
                                int64_t y_row_off, void* y_prev_rank, void* y_next_rank, int64_t frame_rows, void* stream);
 
+/* hi3d_groupnorm_apply_stats with a dense e4m3 output y [rows, C1+C2] (no halo): each value is the fp16 value
+ * hi3d_groupnorm_apply_stats stores, converted with cvt.rn.satfinite.e4m3x2.f16x2 (nearest even, saturating to +-448).  The
+ * producer of an e4m3 GEMM operand (hi3d_gemm_tc5_fp8). */
+int hi3d_groupnorm_apply_stats_fp8(const void* x1, int C1, const float* stats1, const void* x2, int C2, const float* stats2,
+                                   int unit, int n_samples, int64_t rows_per_sample, int imgs_per_sample, int64_t count_rows,
+                                   const float* gamma, const float* beta, float eps, int apply_silu, void* y, void* stream);
+
 /* Frame-sharded runs, where the temporal ResBlock's GroupNorm reduces over (C/32, T, H, W) with T split over GPUs
  * (SURVEY F9): hi3d_groupnorm_group_sums folds unit tables into `sums` fp32 [n_samples, 32, 2] of the local rows; the host
  * all-reduces them over ranks and hi3d_groupnorm_apply_halo normalises with count_rows = the GLOBAL rows per sample.
@@ -165,6 +184,10 @@ int hi3d_groupnorm_apply_halo(const void* x1, int C1, const void* x2, int C2, in
  * Replaces nn.LayerNorm at attention.py:520-522, video_attention.py:51,79,93-94.  y fp16 [M, C]. */
 int hi3d_layernorm(const void* x, const void* addvec, int add_div, int add_mod, int64_t M, int C, const float* gamma,
                    const float* beta, float eps, void* y, void* stream);
+/* hi3d_layernorm with an e4m3 output y [M, C]: each value is the fp16 value hi3d_layernorm stores, converted with
+ * cvt.rn.satfinite.e4m3x2.f16x2 (nearest even, saturating to +-448). */
+int hi3d_layernorm_fp8(const void* x, const void* addvec, int add_div, int add_mod, int64_t M, int C, const float* gamma,
+                       const float* beta, float eps, void* y, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Attention

@@ -34,7 +34,9 @@ from hi3d_official_b200.engine import create_model
 from hi3d_official_b200.util import get_obj_from_str
 
 
-def load_model(config_path, ckpt, stage, tiny=False):
+def load_model(config_path, ckpt, stage, tiny=False, precision="fp16"):
+    """The stage's DiffusionEngine on the GPU; `precision` = operand precision of the denoising UNet's GEMMs
+    (VideoUNet.set_precision), the VAE and the conditioner towers stay fp16."""
     if os.path.exists(config_path) and not tiny:
         model = create_model(config_path)
     else:
@@ -56,6 +58,7 @@ def load_model(config_path, ckpt, stage, tiny=False):
         print(f"[hi3d-b200] checkpoint {ckpt} not found: SEEDED SYNTHETIC WEIGHTS (outputs are not images)")
         model = model.cuda().half()
         spec.synth_fill_(model, seed=0, fast=True)
+    model.model.diffusion_model.set_precision(precision)
     return model
 
 
@@ -169,6 +172,9 @@ def add_cli_args(ap, stage):
     ap.add_argument("--seed", type=int, nargs="+", default=None)
     ap.add_argument("--batch", type=int, default=1,
                     help="objects per sampling batch (several images): trades device memory for throughput, same results")
+    ap.add_argument("--precision", choices=("fp16", "fp8"), default="fp16",
+                    help="operand precision of the denoising UNet's convolutions, projections and feed-forwards: fp8 runs them "
+                         "on e4m3 tensor cores, which changes the result (the VAE and the conditioner stay fp16)")
 
 
 def per_image(values, n, flag):
@@ -248,7 +254,7 @@ def main():
     params = ap.parse_args()
     if len(params.image_path) > 1:
         batch_plan(params)                                                       # argument errors before the model loads
-        model = load_model(params.denoise_config, params.denoise_checkpoint, 1, params.tiny)
+        model = load_model(params.denoise_config, params.denoise_checkpoint, 1, params.tiny, params.precision)
         return main_batch(params, model, model.num_samples, 16 if params.tiny else 64)
     image_path, elevation = params.image_path[0], params.elevation[0]
     towers = params.towers[0] if params.towers else None
@@ -256,7 +262,7 @@ def main():
         raise SystemExit("one image takes one --elevation, --seed and --towers value")
     seed = random.randint(0, 65535) if params.seed is None else params.seed[0]   # v01:33-34
     torch.manual_seed(seed)
-    model = load_model(params.denoise_config, params.denoise_checkpoint, 1, params.tiny)
+    model = load_model(params.denoise_config, params.denoise_checkpoint, 1, params.tiny, params.precision)
     T = model.num_samples                                                        # 16 frames
     h = 16 if params.tiny else 64                                                # 512^2 / 8
     if params.cond:

@@ -101,7 +101,7 @@ def main():
     params = ap.parse_args()
     if len(params.image_path) > 1:
         batch_plan(params)                                                       # argument errors before the model loads
-        model = load_model(params.denoise_config, params.denoise_checkpoint, 2, params.tiny)
+        model = load_model(params.denoise_config, params.denoise_checkpoint, 2, params.tiny, params.precision)
         return main_batch(params, model, model.num_samples, 32 if params.tiny else 128)
     elevation = params.elevation[0]
     towers = params.towers[0] if params.towers else None
@@ -109,7 +109,7 @@ def main():
         raise SystemExit("one image takes one --elevation, --seed and --towers value")
     seed = random.randint(0, 65535) if params.seed is None else params.seed[0]
     torch.manual_seed(seed)
-    model = load_model(params.denoise_config, params.denoise_checkpoint, 2, params.tiny)
+    model = load_model(params.denoise_config, params.denoise_checkpoint, 2, params.tiny, params.precision)
     T = model.num_samples
     h = 32 if params.tiny else 128
     frames = load_first_frames(params.output_dir, T, h, params.synthetic)
