@@ -72,6 +72,10 @@ _SIGS = {
     "hi3d_attention_d64_tc5": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_void_p]),
     "hi3d_attention_tc5_set_exp_emulation": (C.c_int, [C.c_int]),
     "hi3d_attention_tc5_set_variant": (C.c_int, [C.c_int]),
+    "hi3d_attention_vt_e4m3": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "hi3d_attention_vt_e4m3_bytes": (C.c_int64, [C.c_int, C.c_int, C.c_int]),
+    "hi3d_attention_d64_tc5_fp8": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p,
+                                             C.c_void_p]),
     "hi3d_attention_d80_tc5": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_void_p]),
     "hi3d_attention_d512_tc5": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_void_p, C.c_void_p]),
     "hi3d_temporal_attention_d64": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,

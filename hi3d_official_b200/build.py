@@ -20,7 +20,7 @@ INC = os.path.join(os.path.dirname(HERE), "include")
 LIB = os.path.join(HERE, "libhi3d_b200.so")
 STAMP = LIB + ".sha256"                 # digest of what LIB was built from
 OBJ = os.path.join(HERE, "build")
-SOURCES = ["gemm_mma.cu", "gemm_tc5.cu", "attn.cu", "attn_tc5.cu", "norm.cu", "misc.cu", "peer.cu", "attn512_tc5.cu",
+SOURCES = ["gemm_mma.cu", "gemm_tc5.cu", "attn.cu", "attn_tc5.cu", "attn_fp8_tc5.cu", "norm.cu", "misc.cu", "peer.cu", "attn512_tc5.cu",
            "attn_d80_tc5.cu", "dpt.cu", "u2net.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH + ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-I", INC]

@@ -225,6 +225,17 @@ HI3D_DEVINL void wgmma_ss_e4m3<256>(float (&d)[128], uint64_t da, uint64_t db, i
       : "l"(da), "l"(db), "r"(accumulate));
 }
 
+// m64n64k32 e4m3 with A from registers and B from shared memory (K-major): the P V product of the e4m3 attention kernel.  A
+// fragment (PTX ISA, wgmma .m64nNk32 register A for 8-bit types): register r of lane (g = lane / 4, t4 = lane % 4) in warp w
+// holds row 16 w + g + 8 (r & 1), K columns 16 (r >> 1) + 4 t4 + 0..3, lowest byte first.
+HI3D_DEVINL void wgmma_rs_e4m3_64(float (&d)[32], const uint32_t (&a)[4], uint64_t db, int accumulate) {
+  asm volatile(
+      "{\n.reg .pred p;\nsetp.ne.b32 p, %37, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k32.f32.e4m3.e4m3 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1;\n}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate));
+}
+
 // host: encode a tiled tensor map, fp16 and SWIZZLE_128B unless told otherwise (defined in gemm_tc5.cu)
 int encode_map(CUtensorMap* m, const void* ptr, int rank, const cuuint64_t* dims, const cuuint64_t* strides_bytes,
                const cuuint32_t* box, const cuuint32_t* elem_strides,

@@ -271,6 +271,38 @@ def attention_d64(qkv: torch.Tensor, n_img: int, L: int, heads: int, out: torch.
     N.check(fn(qkv.data_ptr(), n_img, L, heads, scale, out.data_ptr(), _stream()), "hi3d_attention_d64")
 
 
+def attention_vt_bytes(n_img: int, L: int, heads: int) -> int:
+    """Size in bytes of attention_vt_e4m3's output (hi3d_attention_vt_e4m3_bytes): n_img * heads * 64 * (L rounded up to 128)."""
+    n = int(N.load().hi3d_attention_vt_e4m3_bytes(n_img, L, heads))
+    if n < 0:
+        N.check(n, "hi3d_attention_vt_e4m3_bytes")
+    return n
+
+
+def attention_vt_e4m3(qkv8: torch.Tensor, n_img: int, L: int, heads: int, vt: torch.Tensor):
+    """V of an e4m3 q|k|v matrix [n_img*L, 3*heads*64] transposed per (image, head) into vt, e4m3 with at least
+    attention_vt_bytes(n_img, L, heads) elements, keys permuted within 32-blocks (layout in include/hi3d_b200.h)."""
+    _chk8(qkv8, "qkv8"); _chk8(vt, "vt")
+    C_ = heads * 64
+    if qkv8.shape[-1] != 3 * C_ or qkv8.numel() < n_img * L * 3 * C_ or vt.numel() < attention_vt_bytes(n_img, L, heads):
+        raise ValueError(f"attention_vt_e4m3: qkv8 {tuple(qkv8.shape)} / vt {tuple(vt.shape)} do not fit {n_img} x {L} x {heads} heads")
+    N.check(N.load().hi3d_attention_vt_e4m3(qkv8.data_ptr(), n_img, L, heads, vt.data_ptr(), _stream()), "hi3d_attention_vt_e4m3")
+
+
+def attention_d64_fp8(qkv8: torch.Tensor, vt: torch.Tensor, n_img: int, L: int, heads: int, out: torch.Tensor,
+                      scale: float = 0.125):
+    """Head dim 64 attention on e4m3 operands (hi3d_attention_d64_tc5_fp8): Q and K from qkv8, V from vt as attention_vt_e4m3
+    wrote it; out fp16 [n_img*L, heads*64]."""
+    _chk8(qkv8, "qkv8"); _chk8(vt, "vt"); _chk16(out, "out")
+    C_ = heads * 64
+    if qkv8.shape[-1] != 3 * C_ or out.shape[-1] != C_ or qkv8.numel() < n_img * L * 3 * C_ or out.numel() < n_img * L * C_ \
+            or vt.numel() < attention_vt_bytes(n_img, L, heads):
+        raise ValueError(f"attention_d64_fp8: qkv8 {tuple(qkv8.shape)} / vt {tuple(vt.shape)} / out {tuple(out.shape)} do not fit "
+                         f"{n_img} x {L} x {heads} heads")
+    N.check(N.load().hi3d_attention_d64_tc5_fp8(qkv8.data_ptr(), vt.data_ptr(), n_img, L, heads, scale, out.data_ptr(), _stream()),
+            "hi3d_attention_d64_tc5_fp8")
+
+
 def attention_d80(qkv: torch.Tensor, n_img: int, L: int, heads: int, out: torch.Tensor, scale: float = 80 ** -0.5):
     """Head dim 80 (OpenCLIP ViT-H/14): qkv fp16 [n_img*L, 3*heads*80] -> out fp16 [n_img*L, heads*80]; any L >= 1."""
     _chk16(qkv, "qkv"); _chk16(out, "out")

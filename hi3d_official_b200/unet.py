@@ -30,7 +30,7 @@ from .spec import Layer, UNetConfig, unet_param_shapes, unet_plan
 
 F16 = torch.float16
 E4M3 = torch.float8_e4m3fn
-PRECISIONS = ("fp16", "fp8")
+PRECISIONS = ("fp16", "fp8", "fp8_attn")
 CIN_PAD = 64     # UNet input channels are zero-padded to one 64-wide K segment per tap
 COUT_PAD = 8     # final conv output channels padded to the engine's N granularity
 
@@ -187,8 +187,10 @@ class VideoUNet(nn.Module):
         """Operand precision of the UNet's large GEMMs.  "fp16" (default): every GEMM in fp16.  "fp8": the ResBlock convs, the
         temporal convs, proj_in, the attention q|k|v projections and the feed-forwards take e4m3 operands (per-output-row weight
         scales, unscaled normalised activations written as e4m3 by their GroupNorm / LayerNorm / GEGLU producers); every other
-        layer stays fp16.  A precision the user chooses, like the sampler: fp8 does not compute what fp16 computes.  Cached
-        plans are dropped, as set_engine does."""
+        layer stays fp16.  "fp8_attn": the fp8 plan, and every spatial self-attention core whose q|k|v GEMM runs in FP8 runs on
+        e4m3 tensor cores too (ops.attention_d64_fp8 on the e4m3 q|k|v that GEMM writes); temporal attention stays fp16.  A
+        precision the user chooses, like the sampler: fp8 does not compute what fp16 computes, nor fp8_attn what fp8 computes.
+        Cached plans are dropped, as set_engine does."""
         if precision not in PRECISIONS:
             raise ValueError(f"precision {precision!r}: expected one of {PRECISIONS}")
         if precision != self.precision:
@@ -348,10 +350,12 @@ class _Plan:
 
     def __init__(self, net: VideoUNet, N: int, H: int, W: int, T: int, shard: Optional[Tuple[int, int]] = None):
         self.shard = None if shard is None or shard[1] == 1 else (int(shard[0]), int(shard[1]))
-        self.fp8 = net.precision == "fp8"
+        self.fp8 = net.precision in ("fp8", "fp8_attn")
+        self.fp8_attn = net.precision == "fp8_attn"
         if self.fp8 and self.shard:
-            raise NotImplementedError("fp8 precision is not built for frame-sharded plans; use fp16")
+            raise NotImplementedError(f"{net.precision} precision is not built for frame-sharded plans; use fp16")
         self.fp8_layers: List[str] = []    # state-dict names of the layers this plan runs with e4m3 operands, in plan order
+        self.fp8_attention: List[str] = []  # spatial BasicTransformerBlocks whose attention core runs on e4m3, in plan order
         self.rank, self.world = self.shard if self.shard else (0, 1)
         self.Tg = T * self.world                     # frames per clip over all ranks
         if N % T:
@@ -770,9 +774,23 @@ class _Plan:
             # ---- spatial BasicTransformerBlock (attention.py:551-572)
             self._ln(bl, tok, P[qs + "norm1"], ln, M)
             Wq, kwq = self._qkv(qs, f8)
-            self._gemm(bl, lambda: [ops.SegSpec(ln.t)], Wq, qkv, M, **kwq)
-            self._call(bl, lambda: ops.attention_d64(qkv.t, N, HW, heads, att.t, engine=self.attn_engine), kind="spatial_attention",
-                       flops=4.0 * N * HW * HW * C, bytes=8.0 * M * C)
+            if self.fp8_attn and f8:
+                # e4m3 attention core: the q|k|v GEMM stores e4m3, V is transposed per (image, head) into vt, and the kernel
+                # reads Q and K from qkv8 and V from vt
+                qkv8 = A.want("qkv8", M, 3 * C, E4M3)
+                vtb = ops.attention_vt_bytes(N, HW, heads)
+                vt = A.want("vt", vtb, 1, E4M3)
+                self._gemm(bl, lambda: [ops.SegSpec(ln.t)], Wq, qkv8, M, **kwq)
+                self._call(bl, lambda: ops.attention_vt_e4m3(qkv8.t, N, HW, heads, vt.t), kind="spatial_attention",
+                           flops=0.0, bytes=float(M * C + vtb))
+                # block / io: which attention this step computes and its buffers (qkv8, out), for tests that check it
+                self._call(bl, lambda: ops.attention_d64_fp8(qkv8.t, vt.t, N, HW, heads, att.t), kind="spatial_attention",
+                           flops=4.0 * N * HW * HW * C, bytes=float(4 * M * C + vtb), block=qs, io=(qkv8, att, N, HW, heads))
+                self.fp8_attention.append(qs)
+            else:
+                self._gemm(bl, lambda: [ops.SegSpec(ln.t)], Wq, qkv, M, **kwq)
+                self._call(bl, lambda: ops.attention_d64(qkv.t, N, HW, heads, att.t, engine=self.attn_engine),
+                           kind="spatial_attention", flops=4.0 * N * HW * HW * C, bytes=8.0 * M * C)
             self.flops += 4.0 * N * HW * HW * C
             self._gemm(bl, lambda: [ops.SegSpec(att.t)], P[qs + "to_out"][0], t1, M, bias=P[qs + "to_out"][1],
                        residual=tok, rowbias=r_s, rb_div=HW, rb_mod=N)

@@ -206,6 +206,28 @@ int hi3d_attention_d64_tc5(const void* qkv, int n_img, int L, int heads, float s
 int hi3d_attention_tc5_set_variant(int variant);
 int hi3d_attention_tc5_set_exp_emulation(int quarters);
 
+/* The same attention with e4m3 (float8_e4m3fn) operands, in two launches.
+ *
+ * hi3d_attention_vt_e4m3 writes V in the layout FP8 wgmma needs for P V (B K-major, i.e. keys contiguous):
+ *   qkv8: e4m3 [n_img*L, 3*C] (q | k | v column blocks, C = heads*64), as the q|k|v GEMM writes it, unscaled;
+ *   vt:   e4m3 [n_img, heads, 64, Lp], Lp = L rounded up to a multiple of 128.  Row (i, h, d) holds V column h*64 + d of
+ *         image i, one byte per key, with the keys permuted inside every aligned block of 32 columns: column 32*b + k holds
+ *         key 32*b + pi(k), pi(k) = (k & 16) + 8*((k >> 1) & 1) + 2*((k >> 2) & 3) + (k & 1).  Columns whose key is >= L are
+ *         written as zero on every call.
+ *   pi makes the f32 S accumulator fragment of a thread (keys 8i + 2*t4 + {0, 1}) coincide with its e4m3 A fragment of
+ *   the k32 P V product (K columns 4*t4 + 0..3 and 16 + 4*t4 + 0..3).  The caller owns vt; its size in bytes is
+ *   hi3d_attention_vt_e4m3_bytes (negative for bad arguments).
+ *
+ * hi3d_attention_d64_tc5_fp8 computes out fp16 [n_img*L, C] = softmax(Q K^T * scale) V per (image, head) from qkv8's Q and K
+ * and vt's V.  Any L >= 1 and any number of images; rows of out past n_img*L are not touched.  S is accumulated by the FP8
+ * tensor cores (reduced-precision accumulation), the softmax runs in fp32 with scale applied there, P is scaled by 2^8 and
+ * rounded to e4m3 for P V, and the fp32 row sum comes from the unrounded P.  Not the result of hi3d_attention_d64_tc5 on
+ * dequantised inputs: P's e4m3 rounding is a relative 2^-4. */
+int hi3d_attention_vt_e4m3(const void* qkv8, int n_img, int L, int heads, void* vt, void* stream);
+int64_t hi3d_attention_vt_e4m3_bytes(int n_img, int L, int heads);
+int hi3d_attention_d64_tc5_fp8(const void* qkv8, const void* vt, int n_img, int L, int heads, float scale, void* out,
+                               void* stream);
+
 /* Same contract for head dim 80 (C = heads*80): the OpenCLIP ViT-H/14 image tower's attention (open_clip transformer.py
  * nn.MultiheadAttention, 16 heads of 80; the conditioner's FrozenOpenCLIPImageEmbedder, modules.py:570-728).  Any L >= 1;
  * keys of the next image are masked.  TMA + wgmma, with each 80-column head row staged as a 64-column SWIZZLE_128B box plus a

@@ -172,9 +172,10 @@ def add_cli_args(ap, stage):
     ap.add_argument("--seed", type=int, nargs="+", default=None)
     ap.add_argument("--batch", type=int, default=1,
                     help="objects per sampling batch (several images): trades device memory for throughput, same results")
-    ap.add_argument("--precision", choices=("fp16", "fp8"), default="fp16",
+    ap.add_argument("--precision", choices=("fp16", "fp8", "fp8_attn"), default="fp16",
                     help="operand precision of the denoising UNet's convolutions, projections and feed-forwards: fp8 runs them "
-                         "on e4m3 tensor cores, which changes the result (the VAE and the conditioner stay fp16)")
+                         "on e4m3 tensor cores, which changes the result (the VAE and the conditioner stay fp16); fp8_attn "
+                         "also runs every spatial self-attention core on e4m3 tensor cores, which changes the result again")
 
 
 def per_image(values, n, flag):

@@ -4,10 +4,12 @@ x heads: 16384 x 5, 4096 x 10, 1024 x 20, 256 x 20).  Each measurement is CUDA e
 fill --window seconds, after warm-up.  Several libraries (--lib, any build of libhi3d_b200.so with the same C signature,
 e.g. one built from an earlier commit) are timed in one process, alternating between them over --rounds rounds, so that
 clock and power drift hits them alike.  --variants / --emus sweep hi3d_attention_tc5_set_variant and
-hi3d_attention_tc5_set_exp_emulation; without them each library runs its own default.  Prints one JSON line with the
-card's name, power limit and max SM clock beside the times.
+hi3d_attention_tc5_set_exp_emulation; without them each library runs its own default.  --fp8 adds, for every library, the e4m3
+path (hi3d_attention_vt_e4m3 + hi3d_attention_d64_tc5_fp8, reported as "fp8_path") and its kernel alone ("fp8_kernel"),
+alternated with the fp16 kernel in the same rounds, on the same (e4m3-representable) values; every entry's TFLOP/s counts the
+same 4 L^2 C n_img.  Prints one JSON line with the card's name, power limit and max SM clock beside the times.
 
-    python tools/time_attention.py [--lib PATH ...] [--rounds 3] [--window 1.0] [--variants 0,6] [--emus 0,1]
+    python tools/time_attention.py [--lib PATH ...] [--rounds 3] [--window 1.0] [--variants 0,6] [--emus 0,1] [--fp8]
 """
 import argparse
 import ctypes as C
@@ -40,6 +42,14 @@ def load(path):
         getattr(lib, f).restype = C.c_int
         getattr(lib, f).argtypes = [C.c_int]
     lib.hi3d_last_error.restype = C.c_char_p
+    if hasattr(lib, "hi3d_attention_d64_tc5_fp8"):
+        lib.hi3d_attention_vt_e4m3.restype = C.c_int
+        lib.hi3d_attention_vt_e4m3.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]
+        lib.hi3d_attention_vt_e4m3_bytes.restype = C.c_int64
+        lib.hi3d_attention_vt_e4m3_bytes.argtypes = [C.c_int, C.c_int, C.c_int]
+        lib.hi3d_attention_d64_tc5_fp8.restype = C.c_int
+        lib.hi3d_attention_d64_tc5_fp8.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_float, C.c_void_p,
+                                                   C.c_void_p]
     return lib
 
 
@@ -57,6 +67,7 @@ def main():
     ap.add_argument("--shapes", default=",".join(SHAPES))
     ap.add_argument("--variants", help="comma-separated hi3d_attention_tc5_set_variant values")
     ap.add_argument("--emus", help="comma-separated hi3d_attention_tc5_set_exp_emulation values")
+    ap.add_argument("--fp8", action="store_true", help="also time the e4m3 path (transpose + kernel) and its kernel alone")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit("time_attention.py needs a CUDA device")
@@ -67,6 +78,14 @@ def main():
     variants = [int(v) for v in a.variants.split(",")] if a.variants else [None]
     emus = [int(e) for e in a.emus.split(",")] if a.emus else [None]
     configs = [(v, e) for v in variants for e in emus]
+    if a.fp8:
+        missing = [p for p, lib in libs if not hasattr(lib, "hi3d_attention_d64_tc5_fp8")]
+        if missing:
+            sys.exit(f"--fp8: {missing} have no hi3d_attention_d64_tc5_fp8")
+    # entries: (library index, config, what) -- what = "fp16", "fp8_path" or "fp8_kernel"; configs only apply to fp16
+    entries = [(li, cfg, "fp16") for li in range(len(libs)) for cfg in configs]
+    if a.fp8:
+        entries += [(li, (None, None), w) for li in range(len(libs)) for w in ("fp8_path", "fp8_kernel")]
     stream = torch.cuda.current_stream()
     res = {"gpu": card(), "rounds": a.rounds, "window_s": a.window, "libs": a.lib, "results": []}
 
@@ -82,43 +101,56 @@ def main():
         C_ = heads * 64
         g = torch.Generator(device="cuda").manual_seed(1)
         qkv = torch.randn(n_img * L, 3 * C_, device="cuda", generator=g).half()
+        qkv8 = None
+        if a.fp8:       # both paths see the same values: e4m3 for the e4m3 path, the same values in fp16 for the fp16 kernel
+            qkv8 = qkv.to(torch.float8_e4m3fn)
+            qkv = qkv8.half()
+            vt = torch.empty(int(libs[0][1].hi3d_attention_vt_e4m3_bytes(n_img, L, heads)), dtype=torch.uint8, device="cuda")
         out = torch.empty(n_img * L, C_, device="cuda", dtype=torch.float16)
         flop = 4.0 * n_img * heads * L * L * 64
+        st = C.c_void_p(stream.cuda_stream)
 
-        def call(lib):
-            check(lib, lib.hi3d_attention_d64_tc5(qkv.data_ptr(), n_img, L, heads, 0.125, out.data_ptr(),
-                                                  C.c_void_p(stream.cuda_stream)), "hi3d_attention_d64_tc5")
+        def call(lib, what):
+            if what == "fp16":
+                check(lib, lib.hi3d_attention_d64_tc5(qkv.data_ptr(), n_img, L, heads, 0.125, out.data_ptr(), st),
+                      "hi3d_attention_d64_tc5")
+                return
+            if what == "fp8_path":
+                check(lib, lib.hi3d_attention_vt_e4m3(qkv8.data_ptr(), n_img, L, heads, vt.data_ptr(), st), "hi3d_attention_vt_e4m3")
+            check(lib, lib.hi3d_attention_d64_tc5_fp8(qkv8.data_ptr(), vt.data_ptr(), n_img, L, heads, 0.125, out.data_ptr(), st),
+                  "hi3d_attention_d64_tc5_fp8")
 
-        def timed(lib, n):
+        def timed(lib, what, n):
             t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             t0.record()
             for _ in range(n):
-                call(lib)
+                call(lib, what)
             t1.record()
             torch.cuda.synchronize()
             return t0.elapsed_time(t1) / n
 
-        # warm-up and the call count of every (library, config): enough calls to fill the window
+        # warm-up and the call count of every entry: enough calls to fill the window
         calls, times = {}, {}
-        for li, (_, lib) in enumerate(libs):
-            for cfg in configs:
-                setup(lib, cfg)
-                for _ in range(a.warmup):
-                    call(lib)
-                calls[li, cfg] = max(3, int(a.window * 1e3 / timed(lib, 3)) + 1)
-                times[li, cfg] = []
+        for e in entries:
+            li, cfg, what = e
+            lib = libs[li][1]
+            setup(lib, cfg)
+            for _ in range(a.warmup):
+                call(lib, "fp8_path" if what == "fp8_kernel" else what)
+            calls[e] = max(3, int(a.window * 1e3 / timed(lib, what, 3)) + 1)
+            times[e] = []
         for _ in range(a.rounds):
-            for li, (_, lib) in enumerate(libs):
-                for cfg in configs:
-                    setup(lib, cfg)
-                    times[li, cfg].append(timed(lib, calls[li, cfg]))
-        for (li, cfg), ts in times.items():
+            for e in entries:
+                li, cfg, what = e
+                setup(libs[li][1], cfg)
+                times[e].append(timed(libs[li][1], what, calls[e]))
+        for (li, cfg, what), ts in times.items():
             ms = sorted(ts)[len(ts) // 2]
-            res["results"].append({"shape": name, "n_img": n_img, "L": L, "heads": heads, "lib": li,
-                                   "variant": cfg[0], "emu": cfg[1], "calls": calls[li, cfg], "ms": round(ms, 4),
+            res["results"].append({"shape": name, "n_img": n_img, "L": L, "heads": heads, "lib": li, "path": what,
+                                   "variant": cfg[0], "emu": cfg[1], "calls": calls[li, cfg, what], "ms": round(ms, 4),
                                    "ms_min": round(min(ts), 4), "ms_max": round(max(ts), 4),
                                    "tflops": round(flop / ms / 1e9, 1)})
-        del qkv, out
+        del qkv, qkv8, out
     print(json.dumps(res))
 
 

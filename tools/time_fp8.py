@@ -1,9 +1,9 @@
 #!/usr/bin/env python
-"""Time the UNet forward in fp16 and fp8 precision (VideoUNet.set_precision) at the stage-1 (32 x 64^2 latents) and stage-2
-(32 x 128^2) shapes of the sampler: the CFG batch of 2 x 16 frames, synthetic weights, one forward = one CUDA-graph replay of the
-launch plan, as the fused sampler step replays it.  The fp16 and fp8 plans are alternated in rounds; each reports the median of the
-timed forwards after warm-up, the split of one eager forward by kind of launch (CUDA events around every launch), and the relative
-L2 difference of the fp8 output against the fp16 output on the same seeded inputs.  The card's name, power limit and maximum SM
+"""Time the UNet forward in fp16, fp8 and fp8_attn precision (VideoUNet.set_precision) at the stage-1 (32 x 64^2 latents) and
+stage-2 (32 x 128^2) shapes of the sampler: the CFG batch of 2 x 16 frames, synthetic weights, one forward = one CUDA-graph replay
+of the launch plan, as the fused sampler step replays it.  The three plans are alternated in rounds; each reports the median of the
+timed forwards after warm-up, the split of one eager forward by kind of launch (CUDA events around every launch; spatial and
+temporal attention apart), and the relative L2 differences of the outputs on the same seeded inputs.  The card's name, power limit and maximum SM
 clock are read in the same run.  Needs a GPU.
 Usage: python tools/time_fp8.py [--stages 1 2] [--rounds 4] [--reps 6] [--json out.json]"""
 import argparse
@@ -20,6 +20,7 @@ sys.path.insert(0, ROOT)
 
 SHAPES = {1: 64, 2: 128}        # latent side per stage (512^2 / 8, 1024^2 / 8); T = 16 frames, CFG batch 2 x 16
 T = 16
+PRECS = ("fp16", "fp8", "fp8_attn")
 
 
 def card():
@@ -65,7 +66,6 @@ def split(plan):
             k = "gemm_fp8" if s.fp8 else "gemm_fp16"
         else:
             k = getattr(s, "kind", "other")
-            k = "attention" if k.endswith("attention") else k
         out[k] = out.get(k, 0.0) + e0.elapsed_time(e1)
     return {k: round(v, 2) for k, v in sorted(out.items())}
 
@@ -82,7 +82,7 @@ def run_stage(stage, rounds, reps):
     y = torch.randn(N // T, cfg.adm_in_channels, device="cuda", generator=g)
     t = torch.full((N,), 0.7, device="cuda")
     plans, graphs = {}, {}
-    for prec in ("fp16", "fp8"):
+    for prec in PRECS:
         net.set_precision(prec)
         p = plans[prec] = net.get_plan(N, h, h, T)      # set_precision drops the cache, the plan object stays alive here
         p.prepare_conditioning(ctx, y)
@@ -96,22 +96,25 @@ def run_stage(stage, rounds, reps):
         graphs[prec].replay()
         torch.cuda.synchronize()
         outs[prec] = p.net_out.t[:, :cfg.out_channels].float().clone()
-    res["rel_l2_fp8_vs_fp16"] = float((outs["fp8"] - outs["fp16"]).norm() / outs["fp16"].norm())
-    times = {"fp16": [], "fp8": []}
-    for prec in ("fp16", "fp8"):
+    for a, b in (("fp8", "fp16"), ("fp8_attn", "fp16"), ("fp8_attn", "fp8")):
+        res[f"rel_l2_{a}_vs_{b}"] = float((outs[a] - outs[b]).norm() / outs[b].norm())
+    times = {prec: [] for prec in PRECS}
+    for prec in PRECS:
         for _ in range(3):
             graphs[prec].replay()
     for _ in range(rounds):
-        for prec in ("fp16", "fp8"):
+        for prec in PRECS:
             for _ in range(reps):
                 e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
                 e0.record(); graphs[prec].replay(); e1.record()
                 e1.synchronize()
                 times[prec].append(e0.elapsed_time(e1))
-    for prec in ("fp16", "fp8"):
+    for prec in PRECS:
         res[prec] = dict(median_ms=round(statistics.median(times[prec]), 2), n=len(times[prec]),
                          min_ms=round(min(times[prec]), 2), max_ms=round(max(times[prec]), 2), split_ms=split(plans[prec]))
     res["speedup"] = round(res["fp16"]["median_ms"] / res["fp8"]["median_ms"], 3)
+    res["speedup_fp8_attn_vs_fp8"] = round(res["fp8"]["median_ms"] / res["fp8_attn"]["median_ms"], 3)
+    res["fp8_attention_blocks"] = len(plans["fp8_attn"].fp8_attention)
     del graphs, plans, net
     torch.cuda.empty_cache()
     return res
@@ -134,7 +137,10 @@ def main():
         print(f"stage {st} ({r['latents']}, {r['fp8_layers']} fp8 layers): fp16 {r['fp16']['median_ms']} ms, fp8 "
               f"{r['fp8']['median_ms']} ms per forward (median of {r['fp8']['n']}), x{r['speedup']}; rel. L2 fp8 vs fp16 "
               f"{r['rel_l2_fp8_vs_fp16']:.3e}")
-        for prec in ("fp16", "fp8"):
+        print(f"  fp8_attn ({r['fp8_attention_blocks']} e4m3 attention blocks): {r['fp8_attn']['median_ms']} ms, x"
+              f"{r['speedup_fp8_attn_vs_fp8']} vs fp8; rel. L2 vs fp16 {r['rel_l2_fp8_attn_vs_fp16']:.3e}, vs fp8 "
+              f"{r['rel_l2_fp8_attn_vs_fp8']:.3e}")
+        for prec in PRECS:
             print(f"  {prec} split (one eager forward, ms): {r[prec]['split_ms']}")
     print(f"card: {res['card']}")
     if a.json:
