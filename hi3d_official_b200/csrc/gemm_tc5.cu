@@ -24,6 +24,7 @@
 #include <cuda_fp8.h>
 #include <stdlib.h>
 #include <string.h>
+#include <type_traits>
 
 #include "common.cuh"
 #include "tc5.cuh"
@@ -49,6 +50,16 @@ template <> struct T5Op<__nv_fp8_e4m3> {
   static constexpr int ROW = 64, MAX_STAGES = 16;
   static constexpr CUtensorMapDataType DT = CU_TENSOR_MAP_DATA_TYPE_UINT8;
   static constexpr CUtensorMapSwizzle SW = CU_TENSOR_MAP_SWIZZLE_64B;
+};
+
+// FP8 accumulation: a wgmma chain covers T5_PROMOTE k-tiles (128 K elements, 4 k32 steps) before it is added into fp32
+// registers.  Of 2, 4 and 8 k-tiles, 2 measured both the most accurate and the fastest (8 holds the whole ring of 8 stages).
+// The chain runs on CW-column slices of the tile: the whole tile where the accumulator and the chain's registers fit the 168
+// registers of the single-tile kernels (BN <= 128) or the pair kernel's 96 (BN = 64), else half of it (BN = 192) or 32 columns
+// (BN = 256, and pairs at BN = 128).
+constexpr int T5_PROMOTE = 2;
+template <int BN, int NT> struct T5PromoteCols {
+  static constexpr int value = NT == 2 ? (BN == 128 ? 32 : BN) : (BN == 192 ? 96 : (BN == 256 ? 32 : BN));
 };
 
 struct T5Seg {
@@ -193,19 +204,63 @@ __global__ void __launch_bounds__(128 + 256 * NT, 1) gemm_tc5_kernel(const __gri
   float acc[BN / 2];
 #pragma unroll
   for (int i = 0; i < BN / 2; i++) acc[i] = 0.f;
-  {
+  if constexpr (FP8) {
+    // FP8 wgmma adds its products into the accumulator with reduced precision, relative to the accumulator's magnitude: one
+    // chain over a long K loses the late products' low bits against the running sum (measured on an H100: up to 549 x 2^-10
+    // sum |a w| at K = 23040 when one large product comes first).  So each chain covers T5_PROMOTE k-tiles in `part`, which is
+    // then added into the fp32 `acc`.  A chain runs over a slice of CW of the tile's columns at a time, so that acc and part fit
+    // the registers; the slicing does not change any column's arithmetic, and every tile width and pair mode computes the same
+    // bits.
+    constexpr int CW = T5PromoteCols<BN, NT>::value;
+    float part[CW / 2];
+    uint32_t s = 0, ph = 0;
+    // one interval: NK k-tiles from stage s, chained per slice and added into acc; then its stages go back to the producer
+    auto interval = [&](auto nk_) {
+      constexpr int NK = decltype(nk_)::value;
+      {
+        uint32_t s1 = s, ph1 = ph;
+#pragma unroll
+        for (int i = 0; i < NK; i++) {
+          mbar_wait(bar_full + 8 * s1, ph1);
+          if (++s1 == (uint32_t)STAGES) { s1 = 0; ph1 ^= 1; }
+        }
+      }
+#pragma unroll
+      for (int c = 0; c < BN / CW; c++) {
+        wgmma_fence();
+        uint32_t s1 = s;
+#pragma unroll
+        for (int i = 0; i < NK; i++) {
+          const uint64_t ad = gmma_desc_sw64(base + s1 * stage_bytes + cw * 64 * ROW);
+          const uint64_t bd = gmma_desc_sw64(base + s1 * stage_bytes + NT * A_BYTES + c * CW * ROW);
+#pragma unroll
+          for (int k = 0; k < T5_BK / 32; k++)   // +32 bytes along K inside the 64-byte swizzle atom
+            wgmma_ss_e4m3<CW>(part, ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), (i | k) ? 1 : 0);
+          if (++s1 == (uint32_t)STAGES) s1 = 0;
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(part);
+#pragma unroll
+        for (int i = 0; i < CW / 2; i++) acc[c * (CW / 2) + i] += part[i];
+      }
+#pragma unroll
+      for (int i = 0; i < NK; i++) {
+        if (lane == 0) mbar_arrive(bar_empty + 8 * s);
+        if (++s == (uint32_t)STAGES) { s = 0; ph ^= 1; }
+      }
+    };
+    int kt = 0;
+    for (; kt + T5_PROMOTE <= KT; kt += T5_PROMOTE) interval(std::integral_constant<int, T5_PROMOTE>());
+    for (; kt < KT; kt++) interval(std::integral_constant<int, 1>());   // the last KT % T5_PROMOTE k-tiles one by one
+  } else {
     uint32_t s = 0, ph = 0, ps = 0;
     for (int kt = 0; kt < KT; kt++) {
       mbar_wait(bar_full + 8 * s, ph);
       const uint32_t sA = base + s * stage_bytes + cw * 64 * ROW;
       const uint32_t sB = base + s * stage_bytes + NT * A_BYTES;
       wgmma_fence();
-      if constexpr (FP8) {
-        const uint64_t ad = gmma_desc_sw64(sA), bd = gmma_desc_sw64(sB);
-#pragma unroll
-        for (int k = 0; k < T5_BK / 32; k++)   // +32 bytes along K inside the 64-byte swizzle atom
-          wgmma_ss_e4m3<BN>(acc, ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), (kt | k) ? 1 : 0);
-      } else {
+      {
         const uint64_t ad = gmma_desc_sw128(sA), bd = gmma_desc_sw128(sB);
 #pragma unroll
         for (int k = 0; k < T5_BK / 16; k++)   // +32 bytes along K inside the 128-byte swizzle atom

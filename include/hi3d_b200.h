@@ -108,9 +108,10 @@ int hi3d_gemm_tc5(const hi3d_gemm_params* p, void* stream);
 int hi3d_gemm_tc5_set_pair_mode(int mode);
 int hi3d_gemm_tc5_set_epilogue_warps(int warps);
 /* The same engine with e4m3 (float8_e4m3fn) operands: every segment source and W are e4m3, K-major like the fp16 ones (src
- * [rows, ld] with ld a multiple of 16, W [N, K]); wgmma k32 with fp32 accumulators.  The epilogue first scales the accumulator
- * of column n by w_scale[n] (fp32 [N], W's dequantisation scale, see pack.pack_e4m3), then applies exactly the fp16 sequence:
- * bias, rowbias, activation, residual, blend (rowbias, residual and blend_x stay fp16).  out_fp8 = 0: out is fp16; 1: out is
+ * [rows, ld] with ld a multiple of 16, W [N, K]); wgmma k32, each chain of 128 K elements added into fp32 accumulators (the
+ * tensor cores' own FP8 accumulation has reduced precision), in the same order at every tile.  The epilogue first scales the
+ * accumulator of column n by w_scale[n] (fp32 [N], W's dequantisation scale, see pack.pack_e4m3), then applies exactly the fp16
+ * sequence: bias, rowbias, activation, residual, blend (rowbias, residual and blend_x stay fp16).  out_fp8 = 0: out is fp16; 1: out is
  * e4m3, each value the fp16 result converted with cvt.rn.satfinite (nearest even, saturating to +-448).  Tile width, tile pairs
  * and the hooks above follow the fp16 rules.  There is no other e4m3 engine: a geometry this one does not cover (see
  * hi3d_gemm_tc5) returns an error. */
@@ -221,8 +222,8 @@ int hi3d_attention_tc5_set_exp_emulation(int quarters);
  * hi3d_attention_d64_tc5_fp8 computes out fp16 [n_img*L, C] = softmax(Q K^T * scale) V per (image, head) from qkv8's Q and K
  * and vt's V.  Any L >= 1 and any number of images; rows of out past n_img*L are not touched.  S is accumulated by the FP8
  * tensor cores (reduced-precision accumulation), the softmax runs in fp32 with scale applied there, P is scaled by 2^8 and
- * rounded to e4m3 for P V, and the fp32 row sum comes from the unrounded P.  Not the result of hi3d_attention_d64_tc5 on
- * dequantised inputs: P's e4m3 rounding is a relative 2^-4. */
+ * rounded to e4m3 for P V, each 128-key tile's P V is added into fp32 O registers, and the fp32 row sum comes from the
+ * unrounded P.  Not the result of hi3d_attention_d64_tc5 on dequantised inputs: P's e4m3 rounding is a relative 2^-4. */
 int hi3d_attention_vt_e4m3(const void* qkv8, int n_img, int L, int heads, void* vt, void* stream);
 int64_t hi3d_attention_vt_e4m3_bytes(int n_img, int L, int heads);
 int hi3d_attention_d64_tc5_fp8(const void* qkv8, const void* vt, int n_img, int L, int heads, float scale, void* out,

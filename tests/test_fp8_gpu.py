@@ -95,7 +95,8 @@ def _w8(N, K, g):
 def _check(out, ref, absprod, what, fp8_out=False):
     """ref: the fp32 result; absprod: sum_k |a_k w_k| per output, the scale of the accumulation error.  Hopper's e4m3 MMA adds
     products into an accumulator of reduced precision before the fp32 accumulate, so the accumulation-order term is
-    2^-10 of that sum rather than fp32 rounding."""
+    2^-10 of that sum rather than fp32 rounding.  Returns the worst error / tolerance (fp16 output) or the most e4m3 steps
+    from e4m3(reference) (e4m3 output): 1 at most."""
     torch.cuda.synchronize()
     if fp8_out:
         # at most one e4m3 step from e4m3(reference): compare the codes as signed magnitudes
@@ -106,12 +107,14 @@ def _check(out, ref, absprod, what, fp8_out=False):
         # where the accumulation error is below 1/16 of |result|, it is below one e4m3 step (results smaller than that are
         # dominated by the accumulation error, and the fp16-output cases bound it)
         d = d[ref.abs() > 2 ** -6 * absprod]
-        assert int(d.max()) <= 1, f"{what}: e4m3 output {int(d.max())} steps from e4m3(reference)"
-        return
+        steps = int(d.max()) if d.numel() else 0
+        assert steps <= 1, f"{what}: e4m3 output {steps} steps from e4m3(reference)"
+        return float(steps)
     err = (out.float() - ref).abs()
     tol = 2e-3 * ref.abs() + 2 ** -10 * absprod + 1e-3 * float(ref.abs().mean())   # fp16 rounding of output and epilogue
     bad = err > tol
     assert not bool(bad.any()), f"{what}: {int(bad.sum())} outside, max err {float(err.max()):.3e}"
+    return float((err / tol.clamp_min(1e-30)).max())
 
 
 def _epilogue(acc, bias, rowbias, rb_div, act, residual, blend_x, alpha):
@@ -127,29 +130,144 @@ def _epilogue(acc, bias, rowbias, rb_div, act, residual, blend_x, alpha):
     return v
 
 
-# (M, N, pair mode): the tile each shape selects on an H100 (132 SMs) by the engine's cost model, waves x (tile width + 48).
-# Single tiles, M = 132 row tiles: N = 256 / 192 / 128 / 64 -> the 256 / 192 / 128 / 64-wide tile (e.g. N = 192: 1 wave x 240
-# beats 2 x 176 and 3 x 112).  Pairs: M = 264 row tiles (132 pairs), N = 128 -> 128 wide (1 x 176 beats 2 x 112); M = 132 row
-# tiles (66 pairs), N = 64 -> 64 wide.
-PLAIN_SHAPES = [(16896, 256, 0), (16896, 192, 0), (16896, 128, 0), (16896, 64, 0), (33792, 128, 1), (16896, 64, 1),
-                (300, 320, -1), (77, 64, -1)]
+# ---- which tile the engine runs -------------------------------------------------------------------------------------------------
+def sm_count() -> int:
+    return torch.cuda.get_device_properties(0).multi_processor_count
 
 
-@pytest.mark.parametrize("M,N,pair", PLAIN_SHAPES)
-def test_gemm_fp8_plain_tiles(M, N, pair):
-    g = torch.Generator().manual_seed(M + N)
+def tc5_m_tiles(mode: int, M: int, Ho: int = 1, Wo: int = 1, T: int = 1) -> int:
+    """Row tiles of a GEMM on the wgmma engine (tc5_geometry in gemm_tc5.cu): 128 rows, a (tn x th x tw) conv patch or a
+    (tf frames x ts pixels) temporal patch per tile."""
+    if mode == ops.ROWS_PLAIN:
+        return -(-M // 128)
+    if mode == ops.ROWS_CONV2D:
+        tw = th = 1
+        while tw * 2 <= 16 and Wo % (tw * 2) == 0:
+            tw *= 2
+        while tw * th * 2 <= 128 and Ho % (th * 2) == 0:
+            th *= 2
+        return (Wo // tw) * (Ho // th) * (M // (Ho * Wo)) // (128 // (tw * th))
+    HW, ts = Ho * Wo, 1
+    while ts * 2 <= 128 and HW % (ts * 2) == 0:
+        ts *= 2
+    return (HW // ts) * (T // (128 // ts)) * (M // (HW * T))
+
+
+def tc5_tile(K: int, N: int, m_tiles: int, sms: int, pair: int = -1):
+    """(row tiles per CTA, tile width) that the engine picks (tc5_gemm in gemm_tc5.cu): tile pairs for K >= 1920 with at least
+    four 128 x 128 tiles per SM, unless the pair-mode hook forces one or the other; then the width in {256, 192, 128, 64}
+    ({128, 64} for pairs) with the least waves x (width + 48), ties to the wider tile."""
+    nt = 2 if K >= 1920 and m_tiles * -(-N // 128) >= 4 * sms else 1
+    if pair >= 0:
+        nt = pair + 1
+    units, best = -(-m_tiles // nt), None
+    for bn in (128, 64) if nt == 2 else (256, 192, 128, 64):
+        cost = -(-units * -(-N // bn) // sms) * (bn + 48)
+        if best is None or cost < best[0]:
+            best = (cost, bn)
+    return nt, best[1]
+
+
+def gemm_tile(gm: "ops.Gemm", sms: int):
+    """tc5_tile of a baked GEMM (automatic pair mode)."""
+    p = gm.p
+    return tc5_tile(p.K, p.N, tc5_m_tiles(p.mode, p.M, p.Ho, p.Wo, p.T), sms)
+
+
+# Tile targets (row tiles per CTA, tile width, N): every tile the engine has, and ragged last N tiles (320 = 192 + 128 and
+# 128 + 128 + 64).  Single tiles run with the automatic choice (K < 1920 never pairs), pairs with the hook forcing them.
+TILE_TARGETS = [(1, 256, 256), (1, 192, 192), (1, 128, 128), (1, 64, 64), (1, 192, 320), (2, 128, 128), (2, 64, 64),
+                (2, 128, 320)]
+
+
+def tile_geometry(mode: int, n: int):
+    """(M, geom) of the n-th shape of a family per row mode: plain M = 128 n - 5 (a ragged last row tile); 2 n images of
+    8 x 8 (two-image patches, n tiles); n clips of 16 frames of 64 pixels (two-frame patches, 8 n tiles)."""
+    if mode == ops.ROWS_PLAIN:
+        return 128 * n - 5, {}
+    if mode == ops.ROWS_CONV2D:
+        return 128 * n, dict(Ho=8, Wo=8, Hs=8, Ws=8)
+    return 1024 * n, dict(Ho=64, Wo=1, T=16)
+
+
+def tile_shape(mode: int, nt: int, bn: int, N: int, K: int, sms: int):
+    """The smallest shape of the family that fills at least one wave of CTAs on `sms` SMs and for which the engine's cost
+    model picks (nt, bn): (M, geom, pair mode to run it with)."""
+    pair = 1 if nt == 2 else -1
+    for n in range(1, 64 * sms):
+        M, geom = tile_geometry(mode, n)
+        mt = tc5_m_tiles(mode, M, geom.get("Ho", 1), geom.get("Wo", 1), geom.get("T", 1))
+        if -(-mt // nt) * -(-N // bn) >= sms and tc5_tile(K, N, mt, sms, pair) == (nt, bn):
+            return M, geom, pair
+    raise AssertionError(f"no shape of mode {mode} selects {nt} x {bn} for N = {N} on {sms} SMs")
+
+
+def tc5_launches(fn):
+    """(row tiles per CTA, tile width, operand type) of each wgmma GEMM kernel fn() launches, read from the kernel names that
+    torch.profiler records (gemm_tc5_kernel<BN, NT, Op>, demangled or not); None when the profiler delivers no kernel record
+    (CUPTI drops them in some sessions of a long process)."""
+    from torch.autograd import DeviceType
+    from torch.profiler import ProfilerActivity, profile
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        fn()
+        torch.cuda.synchronize()
+    names = [e.name for e in prof.events() if e.device_type == DeviceType.CUDA]
+    if not names:
+        return None
+    out = []
+    for n in names:
+        m = re.search(r"gemm_tc5_kernel<\s*(\d+)\s*,\s*(\d+)\s*,\s*([\w:]+)\s*>", n)
+        if m:
+            out.append((int(m[2]), int(m[1]), m[3]))
+            continue
+        m = re.search(r"gemm_tc5_kernelILi(\d+)ELi(\d+)E\d+(\w+?)EEv", n)
+        if m:
+            out.append((int(m[2]), int(m[1]), m[3]))
+    assert out, f"no gemm_tc5_kernel among the recorded events {sorted(set(names))[:6]}"
+    return out
+
+
+def assert_launched(launched, want, what=""):
+    """The launched kernels (tc5_launches) are [want]; without profiler events the launch is not cross-checked (printed)."""
+    if launched is None:
+        print(f"[tc5 launch] {what}: the profiler delivered no kernel record, launch of {want} not cross-checked")
+        return
+    assert launched == [want], (what, launched, want)
+
+
+def run_pair_mode(pair: int, fn):
+    """fn() with the engine's pair-mode hook set to `pair` (-1 automatic, 0 single tiles, 1 tile pairs), then automatic."""
+    lib = _native.load()
+    _native.check(lib.hi3d_gemm_tc5_set_pair_mode(pair), "hi3d_gemm_tc5_set_pair_mode")
+    try:
+        return fn()
+    finally:
+        lib.hi3d_gemm_tc5_set_pair_mode(-1)
+
+
+@pytest.mark.parametrize("nt,bn,N", TILE_TARGETS + [(0, 0, 320), (0, 0, 64)])
+def test_gemm_fp8_plain_tiles(nt, bn, N):
+    """Each tile of the engine at a plain-rows shape derived from this device's SM count, the engine's launch checked against the
+    restated cost model; nt = 0: few rows (300 and 77), whatever the engine picks."""
+    sms = sm_count()
     K = 320
+    if nt:
+        M, _, pair = tile_shape(ops.ROWS_PLAIN, nt, bn, N, K, sms)
+    else:
+        M, pair = (300 if N == 320 else 77), -1
+    print(f"[fp8 plain tiles] {sms} SMs: M = {M}, N = {N}, pair mode {pair} -> {tc5_tile(K, N, tc5_m_tiles(ops.ROWS_PLAIN, M), sms, pair)}")
+    g = torch.Generator().manual_seed(M + N)
     a = _a8(M, K, g)
     W8, sc, Wd = _w8(N, K, g)
     bias = torch.randn(N, generator=g).to(DEV)
     out = torch.empty(M, N, dtype=torch.float16, device=DEV)
-    lib = _native.load()
-    try:
-        if pair >= 0:
-            lib.hi3d_gemm_tc5_set_pair_mode(pair)
-        ops.Gemm([ops.SegSpec(a)], W8, out, M, bias=bias, w_scale=sc, engine="tc5")()
-    finally:
-        lib.hi3d_gemm_tc5_set_pair_mode(-1)
+    gm = ops.Gemm([ops.SegSpec(a)], W8, out, M, bias=bias, w_scale=sc, engine="tc5")
+    launched = run_pair_mode(pair, lambda: tc5_launches(gm))
+    want = tc5_tile(K, N, tc5_m_tiles(ops.ROWS_PLAIN, M), sms, pair)
+    assert_launched(launched, want + ("__nv_fp8_e4m3",), f"plain M={M} N={N}")
+    if nt:
+        assert want == (nt, bn)
     _check(out, a.float() @ Wd.t() + bias, a.float().abs() @ Wd.abs().t(), f"plain M={M} N={N} pair={pair}")
 
 
@@ -253,12 +371,12 @@ def _unet(seed=1):
     return net.cuda().half(), {k: v.cuda() for k, v in sd.items()}
 
 
-def _inputs(N, hw, T, seed=0):
+def _inputs(N, hw, T, seed=0, in_channels=8, adm=768):
     g = torch.Generator().manual_seed(seed)
-    x = torch.randn(N, 8, hw, hw, generator=g).cuda()
+    x = torch.randn(N, in_channels, hw, hw, generator=g).cuda()
     ctx = torch.randn(N // T, 1, 1024, generator=g).cuda()
     ctx[0] = 0
-    y = torch.randn(N // T, 768, generator=g).cuda()
+    y = torch.randn(N // T, adm, generator=g).cuda()
     return x, ctx, y, torch.full((N,), 0.7).cuda()
 
 
@@ -359,10 +477,12 @@ def _layer_reference(sd, g, srcs, residual, blend_x, rowbias, skip_ref):
     return y, a
 
 
-def _teacher_forced_mismatches(net, sd, N, hw, T):
+def _teacher_forced_mismatches(net, sd, N, hw, T, inputs=_inputs, seen=None, after=None):
     """Runs the fp8 plan launch by launch; checks each GEMM that computes state-dict layers against _layer_reference with the
-    GEMM tests' tolerance (_check).  Returns [(layer, message)] of the GEMMs outside it."""
-    x, ctx, y, t = _inputs(N, hw, T)
+    GEMM tests' tolerance (_check).  Returns [(layer, message)] of the GEMMs outside it.  inputs(N, hw, T) -> (x, context, y,
+    timesteps); seen: a list that gets (layer, GEMM, _check's ratio or None) of every checked GEMM; after(step): called after
+    every other step."""
+    x, ctx, y, t = inputs(N, hw, T)
     net(x, timesteps=t, context=ctx, y=y, num_video_frames=T)       # conditioning, input and timesteps of the plan
     plan = net.get_plan(N, hw, hw, T)
     bad, skip_ref, checked = [], None, 0
@@ -370,6 +490,8 @@ def _teacher_forced_mismatches(net, sd, N, hw, T):
         layers = getattr(s, "layers", None) if isinstance(s, ops.Gemm) else None
         if layers is None:
             s()
+            if after is not None:
+                after(s)
             continue
         segs, _, out, _, rowbias, residual, blend_x, _ = s._keep
         srcs = list({sg.src.data_ptr(): sg.src for sg in segs}.values())
@@ -382,10 +504,13 @@ def _teacher_forced_mismatches(net, sd, N, hw, T):
             skip_ref = ref
         elif layers[0].endswith("out_layers.3"):
             skip_ref = None
+        ratio = None
         try:
-            _check(out[:s.p.M], ref, absprod, layers[0], fp8_out=out.dtype == E4M3)
+            ratio = _check(out[:s.p.M], ref, absprod, layers[0], fp8_out=out.dtype == E4M3)
         except AssertionError as e:
             bad.append((layers[0], str(e).splitlines()[0]))
+        if seen is not None:
+            seen.append((layers[0], s, ratio))
     assert checked >= len(plan.fp8_layers) // 3
     return bad
 
