@@ -264,9 +264,28 @@ def layernorm(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, y: torch
                _stream()), "hi3d_layernorm_fp8" if y.dtype == E4M3 else "hi3d_layernorm")
 
 
+def attention_shapes(name: str, qkv: torch.Tensor, out: torch.Tensor, n_img: int, L: int, heads: int, d: int,
+                     T: Optional[int] = None, L_multiple: int = 1):
+    """Raise ValueError unless q|k|v and out fit an attention launch: qkv [>= rows, 3 * heads * d] and out
+    [>= rows, heads * d], row stride = last dimension, rows = n_img * L (spatial) or n_img * T * L (temporal: n_img clips of
+    T <= 16 frames and L pixels); L a multiple of L_multiple.  Reads shapes only (CPU and meta tensors work), so a geometry
+    the kernel would read or write past is refused before anything is launched."""
+    if n_img <= 0 or L <= 0 or heads <= 0 or (T is not None and not 1 <= T <= 16):
+        raise ValueError(f"{name}: bad geometry n_img={n_img} L={L} heads={heads}"
+                         + ("" if T is None else f" T={T} (T must be 1 .. 16)"))
+    if L % L_multiple:
+        raise ValueError(f"{name}: L = {L} is not a multiple of {L_multiple}")
+    rows, C_ = n_img * L * (1 if T is None else T), heads * d
+    if qkv.dim() < 1 or qkv.shape[-1] != 3 * C_ or qkv.numel() < rows * 3 * C_:
+        raise ValueError(f"{name}: qkv {tuple(qkv.shape)} does not fit {rows} rows of 3 x {heads} heads x {d}")
+    if out.dim() < 1 or out.shape[-1] != C_ or out.numel() < rows * C_:
+        raise ValueError(f"{name}: out {tuple(out.shape)} does not fit {rows} rows of {heads} heads x {d}")
+
+
 def attention_d64(qkv: torch.Tensor, n_img: int, L: int, heads: int, out: torch.Tensor, scale: float = 0.125,
                   engine: str = "mma"):
     _chk16(qkv, "qkv"); _chk16(out, "out")
+    attention_shapes("attention_d64", qkv, out, n_img, L, heads, 64)
     fn = N.load().hi3d_attention_d64_tc5 if engine == "tc5" else N.load().hi3d_attention_d64
     N.check(fn(qkv.data_ptr(), n_img, L, heads, scale, out.data_ptr(), _stream()), "hi3d_attention_d64")
 
@@ -294,11 +313,9 @@ def attention_d64_fp8(qkv8: torch.Tensor, vt: torch.Tensor, n_img: int, L: int, 
     """Head dim 64 attention on e4m3 operands (hi3d_attention_d64_tc5_fp8): Q and K from qkv8, V from vt as attention_vt_e4m3
     wrote it; out fp16 [n_img*L, heads*64]."""
     _chk8(qkv8, "qkv8"); _chk8(vt, "vt"); _chk16(out, "out")
-    C_ = heads * 64
-    if qkv8.shape[-1] != 3 * C_ or out.shape[-1] != C_ or qkv8.numel() < n_img * L * 3 * C_ or out.numel() < n_img * L * C_ \
-            or vt.numel() < attention_vt_bytes(n_img, L, heads):
-        raise ValueError(f"attention_d64_fp8: qkv8 {tuple(qkv8.shape)} / vt {tuple(vt.shape)} / out {tuple(out.shape)} do not fit "
-                         f"{n_img} x {L} x {heads} heads")
+    attention_shapes("attention_d64_fp8", qkv8, out, n_img, L, heads, 64)
+    if vt.numel() < attention_vt_bytes(n_img, L, heads):
+        raise ValueError(f"attention_d64_fp8: vt {tuple(vt.shape)} does not fit {n_img} x {L} x {heads} heads")
     N.check(N.load().hi3d_attention_d64_tc5_fp8(qkv8.data_ptr(), vt.data_ptr(), n_img, L, heads, scale, out.data_ptr(), _stream()),
             "hi3d_attention_d64_tc5_fp8")
 
@@ -306,9 +323,7 @@ def attention_d64_fp8(qkv8: torch.Tensor, vt: torch.Tensor, n_img: int, L: int, 
 def attention_d80(qkv: torch.Tensor, n_img: int, L: int, heads: int, out: torch.Tensor, scale: float = 80 ** -0.5):
     """Head dim 80 (OpenCLIP ViT-H/14): qkv fp16 [n_img*L, 3*heads*80] -> out fp16 [n_img*L, heads*80]; any L >= 1."""
     _chk16(qkv, "qkv"); _chk16(out, "out")
-    C_ = heads * 80
-    if qkv.shape[-1] != 3 * C_ or out.shape[-1] != C_ or qkv.numel() < n_img * L * 3 * C_ or out.numel() < n_img * L * C_:
-        raise ValueError(f"attention_d80: qkv {tuple(qkv.shape)} / out {tuple(out.shape)} do not fit {n_img} x {L} x {heads} heads")
+    attention_shapes("attention_d80", qkv, out, n_img, L, heads, 80)
     N.check(N.load().hi3d_attention_d80_tc5(qkv.data_ptr(), n_img, L, heads, scale, out.data_ptr(), _stream()),
             "hi3d_attention_d80_tc5")
 
@@ -316,14 +331,15 @@ def attention_d80(qkv: torch.Tensor, n_img: int, L: int, heads: int, out: torch.
 def attention_d512(qkv: torch.Tensor, n_img: int, L: int, out: torch.Tensor, scale: float = 512 ** -0.5):
     """VAE AttnBlock core: one head of dimension 512, qkv fp16 [n_img*L, 1536] -> out fp16 [n_img*L, 512]."""
     _chk16(qkv, "qkv"); _chk16(out, "out")
-    if qkv.shape[-1] != 1536 or out.shape[-1] != 512:
-        raise ValueError("attention_d512: qkv must be [rows, 1536], out [rows, 512]")
+    attention_shapes("attention_d512", qkv, out, n_img, L, 1, 512, L_multiple=128)
     N.check(N.load().hi3d_attention_d512_tc5(qkv.data_ptr(), n_img, L, scale, out.data_ptr(), _stream()), "hi3d_attention_d512_tc5")
 
 
 def temporal_attention_d64(qkv: torch.Tensor, B: int, T: int, S: int, heads: int, out: torch.Tensor,
                            scale: float = 0.125):
+    """qkv fp16 [B * T * S, 3 * heads * 64] -> out fp16 [B * T * S, heads * 64], rows (clip b, frame t, pixel s); T <= 16."""
     _chk16(qkv, "qkv"); _chk16(out, "out")
+    attention_shapes("temporal_attention_d64", qkv, out, B, S, heads, 64, T=T)
     N.check(N.load().hi3d_temporal_attention_d64(qkv.data_ptr(), B, T, S, heads, scale, out.data_ptr(), _stream()),
             "hi3d_temporal_attention_d64")
 
