@@ -52,6 +52,7 @@ _SIGS = {
     "hi3d_gemm_tc5_set_epilogue_warps": (C.c_int, [C.c_int]),
     "hi3d_gemm_tc5_fp8": (C.c_int, [C.POINTER(GemmParams), C.c_void_p, C.c_int, C.c_void_p]),
     "hi3d_gemm_tc5_fp8_covers": (C.c_int, [C.POINTER(GemmParams)]),
+    "hi3d_gemm_tc5_schedule": (C.c_int, [C.POINTER(GemmParams)]),
     "hi3d_groupnorm_apply_stats": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int,
                                              C.c_int64, C.c_int, C.c_int64, C.c_void_p, C.c_void_p, C.c_float, C.c_int,
                                              C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p]),

@@ -4,22 +4,35 @@
 // geometries this engine does not cover (upsample-fused convs, odd patch shapes, N < 32, > 4 distinct A sources) are
 // forwarded to the mma.sync engine.
 //
-// One CTA per 128 x BN output tile (BN in {64, 128, 192, 256}, chosen per call to cover N with the least padding and
-// wave quantisation over the SMs; n-tile fastest so that CTAs running together share A rows through L2).  The 128 rows of
-// a tile are
+// The 128 rows of a tile are
 //   PLAIN    : 128 consecutive rows
 //   CONV2D   : a (tn images) x (th rows) x (tw columns) patch, tn*th*tw = 128 -- the 3x3 taps are the same TMA box
 //              shifted by (dy, dx) and the zero padding is TMA out-of-bounds fill (stride 2: TMA element strides)
 //   TEMPORAL : (tf frames) x (ts pixels), tf*ts = 128 -- the temporal taps shift the frame coordinate of a
 //              [C, HW, T, B] view; clip boundaries zero-fill by OOB.
-// Warp roles (128 + 256 NT threads): warpgroup 0 = TMA producer (one elected thread), then two MMA + epilogue warpgroups
-// per 128-row tile (rows 0..63 and 64..127).  NT = 2 ("tile pairs", 16 epilogue warps) puts two consecutive row tiles in
-// one CTA that share every B tile -- half the B bytes from L2 per output row, for long-K shapes -- and is built for
-// BN <= 128 (the register budget of 640 threads).  The producer hands its registers to the MMA warpgroups (setmaxnreg):
-// a 64 x 256 fp32 accumulator is 128 registers per thread.
-// The kernel is templated on the operand type: hi3d_gemm_tc5 runs fp16 operands and hi3d_gemm_tc5_fp8 e4m3 ones (wgmma k32,
-// SWIZZLE_64B stages, a per-column weight scale on the fp32 accumulator and an optional e4m3 output); the producer, the row
-// mappings and the epilogue are shared.
+// Tiles are ordered n-tile fastest, so that CTAs running together share A rows through L2.  Two schedules share the TMA
+// producer (t5_produce), the row mappings and the epilogue arithmetic (t5_stage, then t5_finish_chunk):
+//
+// gemm_tc5_kernel -- one CTA per 128 x BN output tile (BN in {64, 128, 192, 256}, chosen per call to cover N with the least
+// padding and wave quantisation over the SMs).  Warp roles (128 + 256 NT threads): warpgroup 0 = TMA producer (one elected
+// thread), then two MMA + epilogue warpgroups per 128-row tile (rows 0..63 and 64..127); the epilogue runs after the main loop,
+// in the ring.  NT = 2 ("tile pairs", 16 epilogue warps) puts two consecutive row tiles in one CTA that share every B tile --
+// half the B bytes from L2 per output row, for long-K shapes -- and is built for BN <= 128 (the register budget of 640
+// threads).  The producer hands its registers to the MMA warpgroups (setmaxnreg): a 64 x 256 fp32 accumulator is 128
+// registers per thread.
+//
+// gemm_tc5_pingpong_kernel -- fp16, short K: a persistent grid of min(tiles, SMs) CTAs; one producer fills one ring across all
+// of a CTA's tiles, and two consumer warpgroups take its tiles in turn, each owning a whole 128 x BN tile (BN in {64, 128}) and
+// its own staging tile.  Their MMA turns alternate, so one warpgroup's epilogue runs while the other's main loop has the tensor
+// cores.  With K short the epilogue is as long as the main loop, and the single-tile kernel leaves the tensor cores idle for it.
+//
+// Selection (tc5_choose, the only place): an fp16 GEMM with K <= 64 T5_PINGPONG_MAX_KT, M >= 128 and at least one tile per SM
+// runs ping-pong; otherwise tile pairs for K >= 1920 with 4 pair tiles per SM, else single tiles.  The hooks
+// hi3d_gemm_tc5_set_pair_mode / set_epilogue_warps force single tiles or pairs, and hi3d_gemm_tc5_schedule reports the choice.
+// The kernels are templated on the operand type: hi3d_gemm_tc5 runs fp16 operands and hi3d_gemm_tc5_fp8 e4m3 ones (wgmma k32,
+// SWIZZLE_64B stages, a per-column weight scale on the fp32 accumulator and an optional e4m3 output).  The e4m3 path keeps the
+// single-tile / pair schedule: its chained accumulation (`part`, see T5_PROMOTE) needs registers beside the accumulator that a
+// 128 x 128 consumer tile does not leave.
 #include <cuda.h>
 #include <cuda_fp8.h>
 #include <stdlib.h>
@@ -74,7 +87,7 @@ struct T5Params {
   T5Seg seg[HI3D_MAX_SEGS];
   int nseg;
   int M, N, K, mode;
-  int stages, n_tiles;
+  int stages, n_tiles, m_tiles;   // m_tiles: row tiles (ping-pong schedule's persistent grid)
   // tile -> rows
   int tw, th, tn;      // CONV2D patch (PLAIN: tw = 128, th = tn = 1; TEMPORAL: tw = ts, th = tf)
   int Wo, Ho, Nimg;    // CONV2D: output W, H, images.  TEMPORAL: Wo = HW, Ho = T, Nimg = B
@@ -124,6 +137,144 @@ HI3D_DEVINL long long t5_row(const T5Params& p, int mt, const T5Tile& o, int r) 
   return ((long long)n * p.Ho + y) * p.Wo + x;
 }
 
+// The TMA producer's k-loop over one CTA tile (NT row tiles from mt0, origins o, columns from n0).  The whole calling warp walks
+// the loop with warp-uniform values and one lane issues.  s / ph: ring position and phase, carried from one tile to the next by
+// the persistent kernel.
+template <int BN, int NT, typename Op>
+HI3D_DEVINL void t5_produce(const T5Params& p, uint32_t base, uint32_t bar_full, uint32_t bar_empty, int mt0,
+                            const T5Tile (&o)[NT], int n0, uint32_t& s, uint32_t& ph) {
+  constexpr int ROW = T5Op<Op>::ROW;
+  constexpr int A_BYTES = T5_BM * ROW;
+  constexpr uint32_t stage_bytes = NT * A_BYTES + BN * ROW;
+  const int lane = threadIdx.x & 31, KT = p.K / T5_BK, STAGES = p.stages;
+  int si = 0, so = 0;
+  T5Seg sg = p.seg[0];
+  const CUtensorMap* am = &p.amap[sg.map];
+  for (int kt = 0; kt < KT; kt++) {
+    mbar_wait(bar_empty + 8 * s, ph ^ 1);
+    if (lane == 0) {
+      const uint32_t sB = base + s * stage_bytes + NT * A_BYTES;
+      const uint32_t full = bar_full + 8 * s;
+      const int c = sg.c_off + so;
+      mbar_expect_tx(full, stage_bytes);
+      // a second row tile past the last one loads out of bounds (zeros) and stores nothing
+#pragma unroll
+      for (int t = 0; t < NT; t++) {
+        const uint32_t sA = base + s * stage_bytes + t * A_BYTES;
+        if (p.mode == HI3D_ROWS_PLAIN)
+          tma_load_2d(sA, am, full, c, (mt0 + t) * T5_BM);
+        else if (p.mode == HI3D_ROWS_CONV2D)
+          tma_load_4d(sA, am, full, c, o[t].x0 * p.cstride + sg.dx, o[t].y0 * p.cstride + sg.dy, o[t].z0);
+        else
+          tma_load_4d(sA, am, full, c, o[t].x0, o[t].y0 + p.t_off + sg.dt, o[t].z0);
+      }
+      tma_load_2d(sB, &p.bmap, full, kt * T5_BK, n0);
+    }
+    __syncwarp();
+    so += T5_BK;
+    if (so >= sg.C && kt + 1 < KT) { si++; so = 0; sg = p.seg[si]; am = &p.amap[sg.map]; }
+    if (++s == (uint32_t)STAGES) { s = 0; ph ^= 1; }
+  }
+}
+
+// Epilogue phase 1 for one thread's share of a 64-row accumulator fragment (wgmma m64nBN layout): rows rl and rl + 8 of the
+// staging tile sC (row pitch BN + 8 halfs), global rows m[0] / m[1] (-1 past the end), columns from n0.  In fp32: the e4m3 weight
+// scale, bias, rowbias, then SiLU or GEGLU; one fp16 rounding into sC.
+template <int BN, bool FP8>
+HI3D_DEVINL void t5_stage(const T5Params& p, const float (&acc)[BN / 2], __half* sC, int rl, const long long (&m)[2], int n0) {
+  constexpr int pitch = BN + 8;
+  const bool geglu = (p.act == HI3D_ACT_GEGLU);
+  const int t4 = threadIdx.x & 3;
+#pragma unroll
+  for (int hh = 0; hh < 2; hh++) {
+    const int r = rl + 8 * hh;
+    const __half* rbp = nullptr;
+    if (p.rowbias != nullptr && m[hh] >= 0) rbp = p.rowbias + (long long)((m[hh] / p.rb_div) % p.rb_mod) * p.rb_ld;
+#pragma unroll
+    for (int j = 0; j < BN / 8; j++) {
+      const int cl = j * 8 + 2 * t4;
+      const int n = n0 + cl;
+      float v0 = acc[4 * j + 2 * hh], v1 = acc[4 * j + 2 * hh + 1];
+      if (n < p.N) {
+        if constexpr (FP8) {
+          const float2 ws = __ldg(reinterpret_cast<const float2*>(p.w_scale + n));
+          v0 *= ws.x;
+          v1 *= ws.y;
+        }
+        if (p.bias != nullptr) {
+          v0 += __ldg(p.bias + n);
+          v1 += __ldg(p.bias + n + 1);
+        }
+        if (rbp != nullptr) {
+          const __half2 rbv = *reinterpret_cast<const __half2*>(rbp + n);
+          v0 += __low2float(rbv);
+          v1 += __high2float(rbv);
+        }
+      }
+      if (geglu) {
+        sC[r * pitch + (cl >> 1)] = __float2half_rn(v0 * gelu_erf_f(v1));
+      } else {
+        if (p.act == HI3D_ACT_SILU) {
+          v0 = silu_f(v0);
+          v1 = silu_f(v1);
+        }
+        *reinterpret_cast<uint32_t*>(sC + r * pitch + cl) = pack_half2(v0, v1);
+      }
+    }
+  }
+}
+
+// Epilogue phase 2, split so that a caller can issue the global loads of several chunks before their stores.  out may alias
+// residual or blend_x element for element (an in-place residual add), never partially: a chunk is only read by its own loads.
+// t5_out_row: the output row of global row m (differs from m only for the parity-class upsample convs).
+HI3D_DEVINL long long t5_out_row(const T5Params& p, long long m) {
+  if (!p.out_up) return m;
+  const int hw = p.Ho * p.Wo;
+  const int n_ = (int)(m / hw), rem_ = (int)(m - (long long)n_ * hw);
+  const int y_ = rem_ / p.Wo, x_ = rem_ - y_ * p.Wo;
+  return ((long long)n_ * 2 * p.Ho + 2 * y_ + p.out_py) * (2 * p.Wo) + 2 * x_ + p.out_px;
+}
+HI3D_DEVINL void t5_load_chunk(const T5Params& p, long long mo, int nc, Half8& rr, Half8& xx) {
+  if (p.residual != nullptr) rr = *reinterpret_cast<const Half8*>(p.residual + mo * p.res_ld + nc);
+  if (p.blend_x != nullptr) xx = *reinterpret_cast<const Half8*>(p.blend_x + mo * p.blend_ld + nc);
+}
+// The 8 staged halfs v of output row mo, columns nc .. nc + 7, with that chunk's residual rr / blend xx: the GELU family, then
+// the residual add, then the blend; one coalesced store.
+template <bool FP8>
+HI3D_DEVINL void t5_finish_chunk(const T5Params& p, Half8 v, long long mo, int nc, const Half8& rr, const Half8& xx) {
+  if (p.act >= HI3D_ACT_GELU) store_act_half8(p.act, v);
+  if (p.residual != nullptr) {
+#pragma unroll
+    for (int q = 0; q < 4; q++) {
+      const float2 a = __half22float2(v.h[q]), b = __half22float2(rr.h[q]);
+      v.h[q] = __floats2half2_rn(a.x + b.x, a.y + b.y);
+    }
+  }
+  if (p.blend_x != nullptr) {
+    const float al = p.alpha, be = 1.f - p.alpha;
+#pragma unroll
+    for (int q = 0; q < 4; q++) {
+      const float2 a = __half22float2(v.h[q]), b = __half22float2(xx.h[q]);
+      v.h[q] = __floats2half2_rn(al * b.x + be * a.x, al * b.y + be * a.y);
+    }
+  }
+  if constexpr (FP8) {
+    if (p.out_fp8) {
+      *reinterpret_cast<uint2*>(reinterpret_cast<uint8_t*>(p.out) + mo * p.out_ld + nc) = half8_to_e4m3(v);
+      return;
+    }
+  }
+  *reinterpret_cast<Half8*>(p.out + mo * p.out_ld + nc) = v;
+}
+// One chunk: the 8 staged halfs v of global row m (>= 0), output columns nc .. nc + 7.
+template <bool FP8>
+HI3D_DEVINL void t5_store_chunk(const T5Params& p, Half8 v, long long m, int nc) {
+  const long long mo = t5_out_row(p, m);
+  Half8 rr, xx;
+  t5_load_chunk(p, mo, nc, rr, xx);
+  t5_finish_chunk<FP8>(p, v, mo, nc, rr, xx);
+}
+
 template <int BN, int NT, typename Op>
 __global__ void __launch_bounds__(128 + 256 * NT, 1) gemm_tc5_kernel(const __grid_constant__ T5Params p) {
   constexpr bool FP8 = sizeof(Op) == 1;
@@ -161,35 +312,8 @@ __global__ void __launch_bounds__(128 + 256 * NT, 1) gemm_tc5_kernel(const __gri
     // ======================= TMA producer =======================
     if (NT == 1) setmaxnreg_dec<40>();
     if (tid < 32) {
-      // the whole warp walks the loop with warp-uniform values and one lane issues
       uint32_t s = 0, ph = 0;
-      int si = 0, so = 0;
-      T5Seg sg = p.seg[0];
-      const CUtensorMap* am = &p.amap[sg.map];
-      for (int kt = 0; kt < KT; kt++) {
-        mbar_wait(bar_empty + 8 * s, ph ^ 1);
-        if (lane == 0) {
-          const uint32_t sB = base + s * stage_bytes + NT * A_BYTES;
-          const uint32_t full = bar_full + 8 * s;
-          const int c = sg.c_off + so;
-          mbar_expect_tx(full, stage_bytes);
-          // a second row tile past the last one loads out of bounds (zeros) and stores nothing
-          for (int t = 0; t < NT; t++) {
-            const uint32_t sA = base + s * stage_bytes + t * A_BYTES;
-            if (p.mode == HI3D_ROWS_PLAIN)
-              tma_load_2d(sA, am, full, c, (mt0 + t) * T5_BM);
-            else if (p.mode == HI3D_ROWS_CONV2D)
-              tma_load_4d(sA, am, full, c, o[t].x0 * p.cstride + sg.dx, o[t].y0 * p.cstride + sg.dy, o[t].z0);
-            else
-              tma_load_4d(sA, am, full, c, o[t].x0, o[t].y0 + p.t_off + sg.dt, o[t].z0);
-          }
-          tma_load_2d(sB, &p.bmap, full, kt * T5_BK, n0);
-        }
-        __syncwarp();
-        so += T5_BK;
-        if (so >= sg.C && kt + 1 < KT) { si++; so = 0; sg = p.seg[si]; am = &p.amap[sg.map]; }
-        if (++s == (uint32_t)STAGES) { s = 0; ph ^= 1; }
-      }
+      t5_produce<BN, NT, Op>(p, base, bar_full, bar_empty, mt0, o, n0, s, ph);
     }
     return;
   }
@@ -284,44 +408,11 @@ __global__ void __launch_bounds__(128 + 256 * NT, 1) gemm_tc5_kernel(const __gri
   const int BNo = geglu ? BN / 2 : BN;          // staged tile width
   constexpr int pitch = BN + 8;                 // halfs
   __half* sC = reinterpret_cast<__half*>(smem);
-  const int g = lane >> 2, t4 = lane & 3;
-#pragma unroll
-  for (int hh = 0; hh < 2; hh++) {
-    const int rl = cw * 64 + warp * 16 + g + 8 * hh;
-    const long long m = t5_row(p, mt0 + ct, o[ct], rl - ct * T5_BM);
-    const __half* rbp = nullptr;
-    if (p.rowbias != nullptr && m >= 0) rbp = p.rowbias + (long long)((m / p.rb_div) % p.rb_mod) * p.rb_ld;
-#pragma unroll
-    for (int j = 0; j < BN / 8; j++) {
-      const int cl = j * 8 + 2 * t4;
-      const int n = n0 + cl;
-      float v0 = acc[4 * j + 2 * hh], v1 = acc[4 * j + 2 * hh + 1];
-      if (n < p.N) {
-        if constexpr (FP8) {
-          const float2 ws = __ldg(reinterpret_cast<const float2*>(p.w_scale + n));
-          v0 *= ws.x;
-          v1 *= ws.y;
-        }
-        if (p.bias != nullptr) {
-          v0 += __ldg(p.bias + n);
-          v1 += __ldg(p.bias + n + 1);
-        }
-        if (rbp != nullptr) {
-          const __half2 rbv = *reinterpret_cast<const __half2*>(rbp + n);
-          v0 += __low2float(rbv);
-          v1 += __high2float(rbv);
-        }
-      }
-      if (geglu) {
-        sC[rl * pitch + (cl >> 1)] = __float2half_rn(v0 * gelu_erf_f(v1));
-      } else {
-        if (p.act == HI3D_ACT_SILU) {
-          v0 = silu_f(v0);
-          v1 = silu_f(v1);
-        }
-        *reinterpret_cast<uint32_t*>(sC + rl * pitch + cl) = pack_half2(v0, v1);
-      }
-    }
+  {
+    const int rl = cw * 64 + warp * 16 + (lane >> 2);
+    const T5Tile oc = ct == 0 ? o[0] : o[NT - 1];    // no dynamic index: o stays in registers
+    const long long m[2] = {t5_row(p, mt0 + ct, oc, rl - ct * T5_BM), t5_row(p, mt0 + ct, oc, rl + 8 - ct * T5_BM)};
+    t5_stage<BN, FP8>(p, acc, sC, rl, m, n0);
   }
   named_bar_sync(1, MMA_THREADS);
 
@@ -335,41 +426,159 @@ __global__ void __launch_bounds__(128 + 256 * NT, 1) gemm_tc5_kernel(const __gri
     const int nc = nout0 + c * 8;
     if (nc >= Nout) continue;
     const int t = r / T5_BM;
-    const long long m = t5_row(p, mt0 + t, o[t], r - t * T5_BM);
+    const T5Tile ot = t == 0 ? o[0] : o[NT - 1];   // no dynamic index: o stays in registers
+    const long long m = t5_row(p, mt0 + t, ot, r - t * T5_BM);
     if (m < 0) continue;
-    long long mo = m;                       // output row (differs from m only for the parity-class upsample convs)
-    if (p.out_up) {
-      const int hw = p.Ho * p.Wo;
-      const int n_ = (int)(m / hw), rem_ = (int)(m - (long long)n_ * hw);
-      const int y_ = rem_ / p.Wo, x_ = rem_ - y_ * p.Wo;
-      mo = ((long long)n_ * 2 * p.Ho + 2 * y_ + p.out_py) * (2 * p.Wo) + 2 * x_ + p.out_px;
+    t5_store_chunk<FP8>(p, *reinterpret_cast<const Half8*>(sC + r * pitch + c * 8), m, nc);
+  }
+}
+
+// Ping-pong schedule (fp16 operands, short K): a persistent grid whose CTA c takes tiles c, c + grid, c + 2 grid, ... (tile
+// order as gemm_tc5_kernel's CTA order, n-tile fastest).  Warpgroup 0 is the TMA producer; it fills ONE ring in tile order and
+// never drains it between tiles.  Consumer warpgroups 1 and 2 take the CTA's tiles in turn (local tile j -> warpgroup 1 + j % 2),
+// each owning a whole 128 x BN tile as two m64 wgmma rows per k16 step (BN <= 128: 2 x BN / 2 accumulator registers), with its
+// own staging tile outside the ring.  The MMA turns are ordered by a pair of named barriers: a warpgroup starts the main loop of
+// its next tile only once the other one has issued the whole main loop of the tile before it.  So the main loop of tile j + 1
+// runs on the tensor cores while the epilogue of tile j runs on the other warpgroup.  The ordering is also what keeps the ring's
+// parity waits exact: every k-tile a warpgroup waits for is at most one ring lap ahead of the last one consumed.  Each stage is
+// consumed by exactly one warpgroup, so its empty barrier counts that warpgroup's 4 warps.  The k16 MMA sequence of every output
+// element and the epilogue arithmetic are those of gemm_tc5_kernel: results are bit-identical to it.
+constexpr int T5_PP_BATCH = 4;   // ping-pong epilogue: chunks whose global loads are issued together
+template <int BN>
+__global__ void __launch_bounds__(384, 1) gemm_tc5_pingpong_kernel(const __grid_constant__ T5Params p) {
+  constexpr int ROW = T5Op<__half>::ROW;
+  constexpr int A_BYTES = T5_BM * ROW;
+  constexpr uint32_t stage_bytes = A_BYTES + BN * ROW;
+  constexpr int pitch = BN + 8;                 // halfs per staged row
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t raw = smem_u32(smem_raw);
+  const uint32_t base = (raw + 1023u) & ~1023u;          // SWIZZLE_128B atoms need 1024-byte alignment
+  uint8_t* smem = smem_raw + (base - raw);
+  const int STAGES = p.stages;
+  __half* const staging = reinterpret_cast<__half*>(smem + STAGES * stage_bytes);   // 2 x 128 x pitch halfs
+  const uint32_t bar_full = base + STAGES * stage_bytes + 2 * T5_BM * pitch * (uint32_t)sizeof(__half);
+  const uint32_t bar_empty = bar_full + 8 * T5Op<__half>::MAX_STAGES;
+
+  const int tid = threadIdx.x, lane = tid & 31;
+  const int wg = __shfl_sync(0xffffffffu, tid >> 7, 0);    // provably warp-uniform role index
+  const int KT = p.K / T5_BK;
+  const int tiles = p.m_tiles * p.n_tiles;
+  const int n_local = (tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
+
+  if (tid == 0) {
+    for (int s = 0; s < STAGES; s++) {
+      mbar_init(bar_full + 8 * s, 1);        // the producer's expect_tx arrive
+      mbar_init(bar_empty + 8 * s, 4);       // one arrive per warp of the consuming warpgroup
     }
-    Half8 v = *reinterpret_cast<const Half8*>(sC + r * pitch + c * 8);
-    if (p.act >= HI3D_ACT_GELU) store_act_half8(p.act, v);
-    if (p.residual != nullptr) {
-      const Half8 rr = *reinterpret_cast<const Half8*>(p.residual + mo * p.res_ld + nc);
+    asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
+  }
+  __syncthreads();
+
+  if (wg == 0) {
+    // ======================= TMA producer: every tile of this CTA through one ring =======================
+    setmaxnreg_dec<40>();
+    if (tid < 32) {
+      uint32_t s = 0, ph = 0;
+      for (int j = 0; j < n_local; j++) {
+        const int tile = blockIdx.x + j * gridDim.x;
+        const int mt = tile / p.n_tiles;
+        const T5Tile o[1] = {t5_origin(p, mt)};
+        t5_produce<BN, 1, __half>(p, base, bar_full, bar_empty, mt, o, (tile % p.n_tiles) * BN, s, ph);
+      }
+    }
+    return;
+  }
+
+  // ======================= consumer warpgroups: tiles cw, cw + 2, ... of this CTA =======================
+  setmaxnreg_inc<232>();
+  const int cw = wg - 1;
+  const int warp = (tid >> 5) & 3;       // warp inside the warpgroup: accumulator rows 16 warp .. + 15 of each m64 row
+  __half* const sC = staging + cw * T5_BM * pitch;
+  const bool geglu = (p.act == HI3D_ACT_GEGLU);
+  const int cpr = (geglu ? BN / 2 : BN) / 8;   // 16-byte chunks per staged row
+  const int Nout = geglu ? p.N / 2 : p.N;
+  for (int j = cw; j < n_local; j += 2) {
+    const int tile = blockIdx.x + j * gridDim.x;
+    const int mt = tile / p.n_tiles, n0 = (tile % p.n_tiles) * BN;
+    const T5Tile o = t5_origin(p, mt);
+    float acc[2][BN / 2];
 #pragma unroll
-      for (int q = 0; q < 4; q++) {
-        const float2 a = __half22float2(v.h[q]), b = __half22float2(rr.h[q]);
-        v.h[q] = __floats2half2_rn(a.x + b.x, a.y + b.y);
-      }
-    }
-    if (p.blend_x != nullptr) {
-      const Half8 xx = *reinterpret_cast<const Half8*>(p.blend_x + mo * p.blend_ld + nc);
-      const float al = p.alpha, be = 1.f - p.alpha;
+    for (int h = 0; h < 2; h++)
 #pragma unroll
-      for (int q = 0; q < 4; q++) {
-        const float2 a = __half22float2(v.h[q]), b = __half22float2(xx.h[q]);
-        v.h[q] = __floats2half2_rn(al * b.x + be * a.x, al * b.y + be * a.y);
+      for (int i = 0; i < BN / 2; i++) acc[h][i] = 0.f;
+    // our MMA turn: the other warpgroup has issued the main loop of tile j - 1 (and, before that, every thread of this
+    // warpgroup has finished reading sC for tile j - 2)
+    if (j > 0) named_bar_sync(2 + cw, 256);
+    uint32_t it = (uint32_t)j * KT;
+    uint32_t s = it % STAGES, ph = (it / STAGES) & 1, ps = 0;
+    for (int kt = 0; kt < KT; kt++) {
+      mbar_wait(bar_full + 8 * s, ph);
+      const uint32_t sA = base + s * stage_bytes;
+      wgmma_fence();
+      {
+        const uint64_t ad0 = gmma_desc_sw128(sA), ad1 = gmma_desc_sw128(sA + 64 * ROW);
+        const uint64_t bd = gmma_desc_sw128(sA + A_BYTES);
+#pragma unroll
+        for (int k = 0; k < T5_BK / 16; k++) {   // +32 bytes along K inside the 128-byte swizzle atom
+          wgmma_ss<BN>(acc[0], ad0 + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), (kt | k) ? 1 : 0);
+          wgmma_ss<BN>(acc[1], ad1 + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), (kt | k) ? 1 : 0);
+        }
+      }
+      wgmma_commit();
+      // keep one k-block of MMAs in flight: the previous one has retired, its stage goes back to the producer
+      wgmma_wait<1>();
+      if (kt > 0 && lane == 0) mbar_arrive(bar_empty + 8 * ps);
+      ps = s;
+      if (++s == (uint32_t)STAGES) { s = 0; ph ^= 1; }
+    }
+    // hand the tensor cores to the other warpgroup's next tile, then finish ours
+    if (j + 1 < n_local) named_bar_arrive(2 + (cw ^ 1), 256);
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc[0]);
+    wgmma_fence_regs(acc[1]);
+    if (lane == 0) mbar_arrive(bar_empty + 8 * ps);
+
+    // ---- epilogue phase 1: registers -> (bias, rowbias, activation) -> this warpgroup's fp16 staging tile ----
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      const int rl = h * 64 + warp * 16 + (lane >> 2);
+      const long long m[2] = {t5_row(p, mt, o, rl), t5_row(p, mt, o, rl + 8)};
+      t5_stage<BN, false>(p, acc[h], sC, rl, m, n0);
+    }
+    named_bar_sync(4 + cw, 128);
+
+    // ---- epilogue phase 2: coalesced 16-byte stores with residual / blend ---------------------------
+    const int nout0 = geglu ? n0 / 2 : n0;
+    if (p.residual == nullptr && p.blend_x == nullptr) {
+      for (int idx = tid & 127; idx < T5_BM * cpr; idx += 128) {
+        const int r = idx / cpr, c = idx - r * cpr;
+        const int nc = nout0 + c * 8;
+        if (nc >= Nout) continue;
+        const long long m = t5_row(p, mt, o, r);
+        if (m < 0) continue;
+        t5_store_chunk<false>(p, *reinterpret_cast<const Half8*>(sC + r * pitch + c * 8), m, nc);
+      }
+    } else {
+      // T5_PP_BATCH chunks per thread at a time: their residual / blend loads are all in flight before the first store
+      for (int idx0 = tid & 127; idx0 < T5_BM * cpr; idx0 += 128 * T5_PP_BATCH) {
+        long long mo[T5_PP_BATCH];
+        int nc[T5_PP_BATCH], sofs[T5_PP_BATCH];
+        Half8 rr[T5_PP_BATCH], xx[T5_PP_BATCH];
+#pragma unroll
+        for (int u = 0; u < T5_PP_BATCH; u++) {
+          const int idx = idx0 + u * 128;
+          const int r = idx / cpr, c = idx - r * cpr;
+          nc[u] = nout0 + c * 8;
+          sofs[u] = r * pitch + c * 8;
+          const long long m = (idx < T5_BM * cpr && nc[u] < Nout) ? t5_row(p, mt, o, r) : -1;
+          mo[u] = m < 0 ? -1 : t5_out_row(p, m);
+          if (mo[u] >= 0) t5_load_chunk(p, mo[u], nc[u], rr[u], xx[u]);
+        }
+#pragma unroll
+        for (int u = 0; u < T5_PP_BATCH; u++)
+          if (mo[u] >= 0) t5_finish_chunk<false>(p, *reinterpret_cast<const Half8*>(sC + sofs[u]), mo[u], nc[u], rr[u], xx[u]);
       }
     }
-    if constexpr (FP8) {
-      if (p.out_fp8) {
-        *reinterpret_cast<uint2*>(reinterpret_cast<uint8_t*>(p.out) + mo * p.out_ld + nc) = half8_to_e4m3(v);
-        continue;
-      }
-    }
-    *reinterpret_cast<Half8*>(p.out + mo * p.out_ld + nc) = v;
   }
 }
 
@@ -425,6 +634,60 @@ static int launch_tc5(const T5Params& tp, int grid, int smem, cudaStream_t st) {
   if (ensure_dyn_smem(gemm_tc5_kernel<BN, NT, Op>, smem, attr_done, "hi3d_gemm_tc5")) return -1;
   gemm_tc5_kernel<BN, NT, Op><<<grid, 128 + 256 * NT, smem, st>>>(tp);
   return check_launch("hi3d_gemm_tc5");
+}
+
+template <int BN>
+static int launch_pingpong(const T5Params& tp, int grid, int smem, cudaStream_t st) {
+  static bool attr_done[HI3D_MAX_DEVICES];
+  if (ensure_dyn_smem(gemm_tc5_pingpong_kernel<BN>, smem, attr_done, "hi3d_gemm_tc5")) return -1;
+  gemm_tc5_pingpong_kernel<BN><<<grid, 384, smem, st>>>(tp);
+  return check_launch("hi3d_gemm_tc5");
+}
+
+// The ping-pong schedule runs fp16 GEMMs of at most T5_PINGPONG_MAX_KT k-tiles (K <= 1280).  Measured with tools/time_gemm.py on
+// every shape of the stage-2 UNet forward (H100 80GB HBM3, 700 W), ping-pong against the schedule otherwise chosen: 1.02x to
+// 1.37x faster at K = 320 .. 1280 (5 .. 20 k-tiles); 0.82x and 0.90x at the plan's next K, 1920 (30 k-tiles), and slower
+// at nearly every longer K, where tile pairs halve the B traffic and the epilogue is a small part of a tile.  M >= 128: a GEMM of
+// fewer rows is a stream of W through mostly-padding tiles, which the 256-wide single tiles move in half the tiles.
+constexpr int T5_PINGPONG_MAX_KT = 20;
+
+// Schedules (hi3d_gemm_tc5_schedule returns schedule * 1000 + tile width).
+enum { T5_SCHED_MMA_SYNC = 0, T5_SCHED_SINGLE = 1, T5_SCHED_PAIR = 2, T5_SCHED_PINGPONG = 3 };
+struct T5Choice {
+  int sched, BN, ntile;
+};
+
+// The one place that picks a covered GEMM's schedule and tile width (m_tiles from tc5_geometry).
+template <bool FP8>
+static T5Choice tc5_choose(const hi3d_gemm_params* p, int m_tiles) {
+  const int sm_count = device_sm_count();
+  read_env_once();
+  // tile-N in {64, .., max_bn}.  Cost model = waves of one-CTA-per-SM tiles x time per tile, where a tile costs its MMA columns
+  // plus a fixed term (A-operand traffic / epilogue set-up); this accounts both for the padding of N and for wave quantisation
+  // over the SMs.  Ties go to the wider tile.
+  auto pick_bn = [&](int max_bn, int m_units) {
+    int bn = max_bn;
+    long long best = -1;
+    for (int cand = max_bn; cand >= 64; cand -= 64) {
+      const long long ntl = (p->N + cand - 1) / cand;
+      const long long waves = ((long long)m_units * ntl + sm_count - 1) / sm_count;
+      const long long cost = waves * (cand + 48);
+      if (best < 0 || cost < best) { best = cost; bn = cand; }
+    }
+    return bn;
+  };
+  const bool forced = g_ew_mode > 0 || g_pair_mode >= 0;
+  if (!FP8 && !forced && p->K / T5_BK <= T5_PINGPONG_MAX_KT && p->M >= T5_BM) {
+    const int bn = pick_bn(128, m_tiles);
+    if ((long long)m_tiles * ((p->N + bn - 1) / bn) >= sm_count) return {T5_SCHED_PINGPONG, bn, 1};
+  }
+  // Tile pairs (NT = 2): two row tiles share each B tile, halving the B bytes per output row; worth it once the main loop
+  // dominates (long K) and there are enough tiles to fill the SMs with pairs.  The hooks force either choice.
+  int ntile = (p->K >= 1920 && (long long)m_tiles * ((p->N + 127) / 128) >= 4LL * sm_count) ? 2 : 1;
+  if (g_ew_mode > 0) ntile = g_ew_mode / 8;
+  if (g_pair_mode >= 0) ntile = g_pair_mode + 1;
+  const int bn = pick_bn(ntile == 2 ? 128 : 256, (m_tiles + ntile - 1) / ntile);
+  return {ntile == 2 ? T5_SCHED_PAIR : T5_SCHED_SINGLE, bn, ntile};
 }
 
 }  // namespace hi3d
@@ -527,34 +790,21 @@ static int tc5_gemm(const hi3d_gemm_params* p, const float* w_scale, int out_fp8
     return -2;
   }
 
-  // Tile pairs (NT = 2): two row tiles share each B tile, halving the B bytes per output row; worth it once the main loop
-  // dominates (long K) and there are enough tiles to fill the SMs with pairs.  The hooks force either choice.
-  const int sm_count = device_sm_count();
-  read_env_once();
-  int ntile = (p->K >= 1920 && (long long)m_tiles * ((p->N + 127) / 128) >= 4LL * sm_count) ? 2 : 1;
-  if (g_ew_mode > 0) ntile = g_ew_mode / 8;
-  if (g_pair_mode >= 0) ntile = g_pair_mode + 1;
-  const int m_units = (m_tiles + ntile - 1) / ntile;
-  // tile-N in {64, 128, 192, 256} ({64, 128} for pairs).  Cost model = waves of one-CTA-per-SM tiles x time per tile,
-  // where a tile costs its MMA columns plus a fixed term (A-operand traffic / epilogue set-up); this accounts both for the
-  // padding of N and for wave quantisation over the SMs.  Ties go to the wider tile.
-  int BN = ntile == 2 ? 128 : 256;
-  {
-    long long best = -1;
-    for (int cand = BN; cand >= 64; cand -= 64) {
-      const long long ntl = (p->N + cand - 1) / cand;
-      const long long waves = ((long long)m_units * ntl + sm_count - 1) / sm_count;
-      const long long cost = waves * (cand + 48);
-      if (best < 0 || cost < best) { best = cost; BN = cand; }
-    }
-  }
+  const T5Choice ch = tc5_choose<FP8>(p, m_tiles);
+  const int BN = ch.BN, ntile = ch.ntile;
+  const bool pingpong = ch.sched == T5_SCHED_PINGPONG;
   const int stage_bytes = ntile * T5_BM * ROW + BN * ROW;
-  int stages = T5_SMEM_BUDGET / stage_bytes;
+  // the ping-pong schedule keeps one staging tile per consumer warpgroup outside the ring
+  const int staging_bytes = pingpong ? 2 * T5_BM * (BN + 8) * (int)sizeof(__half) : 0;
+  int stages = (T5_SMEM_BUDGET - staging_bytes) / stage_bytes;
   if (stages > MAX_STAGES) stages = MAX_STAGES;
   tp.stages = stages;
   tp.n_tiles = (p->N + BN - 1) / BN;
-  const long long grid = (long long)m_units * tp.n_tiles;
+  tp.m_tiles = m_tiles;
+  const int m_units = (m_tiles + ntile - 1) / ntile;
+  long long grid = (long long)m_units * tp.n_tiles;
   if (grid > 2147483647LL) { set_error("%s: too many tiles", who); return -2; }
+  if (pingpong && grid > device_sm_count()) grid = device_sm_count();
 
   for (int j = 0; j < nmaps; j++) {
     const cuuint64_t ld = (cuuint64_t)lds[j];
@@ -590,7 +840,11 @@ static int tc5_gemm(const hi3d_gemm_params* p, const float* w_scale, int out_fp8
   tp.out = (__half*)p->out; tp.out_ld = p->out_ld;
   tp.w_scale = w_scale; tp.out_fp8 = out_fp8;
 
-  const int smem = stages * stage_bytes + 16 * MAX_STAGES + 1024;
+  const int smem = stages * stage_bytes + staging_bytes + 16 * MAX_STAGES + 1024;
+  if constexpr (!FP8) {
+    if (pingpong)
+      return BN == 64 ? launch_pingpong<64>(tp, (int)grid, smem, st) : launch_pingpong<128>(tp, (int)grid, smem, st);
+  }
   if (ntile == 2)
     return BN == 64 ? launch_tc5<64, 2, Op>(tp, (int)grid, smem, st) : launch_tc5<128, 2, Op>(tp, (int)grid, smem, st);
   switch (BN) {
@@ -621,4 +875,16 @@ extern "C" int hi3d_gemm_tc5_fp8_covers(const hi3d_gemm_params* p) {
   int lds[T5_MAX_MAPS];
   int m_tiles = 0, nmaps = 0;
   return tc5_geometry(p, tp, m_tiles, srcs, lds, nmaps) ? 1 : 0;
+}
+
+extern "C" int hi3d_gemm_tc5_schedule(const hi3d_gemm_params* p) {
+  int rc = validate_gemm(p, "hi3d_gemm_tc5_schedule");
+  if (rc) return rc;
+  T5Params tp;
+  const void* srcs[T5_MAX_MAPS];
+  int lds[T5_MAX_MAPS];
+  int m_tiles = 0, nmaps = 0;
+  if (!tc5_geometry(p, tp, m_tiles, srcs, lds, nmaps)) return T5_SCHED_MMA_SYNC;
+  const T5Choice ch = tc5_choose<false>(p, m_tiles);
+  return ch.sched * 1000 + ch.BN;
 }

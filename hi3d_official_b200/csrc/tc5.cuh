@@ -116,6 +116,10 @@ HI3D_DEVINL void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u3
 HI3D_DEVINL void named_bar_sync(int id, int threads) {
   asm volatile("bar.sync %0, %1;\n" ::"r"(id), "r"(threads) : "memory");
 }
+// Arrive at a named barrier without waiting for it: the signalling side of a producer / consumer pair of thread groups.
+HI3D_DEVINL void named_bar_arrive(int id, int threads) {
+  asm volatile("bar.arrive %0, %1;\n" ::"r"(id), "r"(threads) : "memory");
+}
 
 // Generated wgmma wrappers (m64nNk16, f16 inputs, f32 accumulators).
 // wgmma_ss: A and B from shared memory, both K-major.  wgmma_rs_tb: A from registers, B from shared memory MN-major.

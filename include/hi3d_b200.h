@@ -120,6 +120,11 @@ int hi3d_gemm_tc5_fp8(const hi3d_gemm_params* p, const float* w_scale, int out_f
  * geometry is read (M, N, mode, Ho, Wo, Hs, Ws, stride, ups, out_up, T, the segments' sources and lds, rowbias alignment), so a
  * launch plan can ask before its buffers exist: leave the pointers NULL and list one segment per distinct source. */
 int hi3d_gemm_tc5_fp8_covers(const hi3d_gemm_params* p);
+/* The schedule and tile width hi3d_gemm_tc5 runs the GEMM described by p with, under the current hooks: schedule * 1000 + tile
+ * width, with schedule 1 = one 128-row tile per CTA, 2 = tile pairs, 3 = ping-pong (a persistent grid, two consumer warpgroups
+ * that take turns on the tensor cores, each epilogue overlapping the other's main loop); 0 = the mma.sync engine (geometry not
+ * covered); negative for malformed parameters.  Host-only: launches nothing. */
+int hi3d_gemm_tc5_schedule(const hi3d_gemm_params* p);
 
 /* Tiny channel counts (UNet input 8|17 ch, VAE image 3 ch / latent 4 ch) are zero-padded to 64 channels by
  * hi3d_sampler_pre / hi3d_nchw_to_nhwc so that the same engine serves input_blocks.0.0 (video_model.py:186-191),
