@@ -97,6 +97,12 @@ _SIGS = {
     "hi3d_sampler_post": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
                                     C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "hi3d_sampler_lincomb4": (C.c_int, [C.c_void_p] * 9 + [C.c_int, C.c_int64, C.c_void_p]),
+    "hi3d_sampler_pre_ex": (C.c_int, [C.c_void_p] * 4 + [C.c_float, C.c_void_p, C.c_void_p] + [C.c_int] * 8
+                            + [C.c_void_p] * 4),
+    "hi3d_sampler_post_ancestral": (C.c_int, [C.c_void_p, C.c_int] + [C.c_void_p] * 4 + [C.c_int, C.c_void_p, C.c_float]
+                                    + [C.c_void_p] * 2 + [C.c_int] * 4 + [C.c_void_p] * 3),
+    "hi3d_sampler_lincomb": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_int, C.c_int,
+                                       C.c_int64, C.c_void_p]),
     "hi3d_renoise_blend": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_float, C.c_int64,
                                      C.c_void_p]),
     "hi3d_nchw_to_nhwc": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float,

@@ -76,6 +76,111 @@ __global__ void sampler_post_kernel(const __half* __restrict__ net, int net_ld, 
   }
 }
 
+// The pre step of every sampler, guider and churn setting: `rows` = 2 (CFG batch, uc half first) or 1 (IdentityGuider, cond
+// rows only).  With eps, the network sees the churned x_hat = x + (eps * s_noise) * sqrt(sigma^2 - sigma_from^2) (EDMSampler,
+// sampling.py:94-97), which the first row of each frame also writes to x_hat_out for the post step.
+template <typename TC>
+__global__ void sampler_pre_ex_kernel(const float* __restrict__ x, const float* __restrict__ sigma,
+                                      const float* __restrict__ sigma_from, const float* __restrict__ eps, float s_noise,
+                                      const TC* __restrict__ cuc, const TC* __restrict__ cc, int rows, int F, int Cx, int Cc,
+                                      int HW, int Cpad, __half* __restrict__ out, float* __restrict__ c_noise_out,
+                                      float* __restrict__ x_hat_out) {
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (long long)rows * F * HW) return;
+  const int n = (int)(idx / HW), pix = (int)(idx - (long long)n * HW);
+  const int f = n % F;
+  const bool cond = rows == 1 || n >= F;
+  const float sg = sigma[f];
+  const float c_in = rsqrtf(sg * sg + 1.f);
+  float churn = 0.f;
+  if (eps) {
+    const float sf = sigma_from[f];
+    churn = sqrtf(sg * sg - sf * sf);
+  }
+  if (pix == 0 && c_noise_out != nullptr) c_noise_out[n] = 0.25f * logf(sg);
+  const TC* cat = cond ? cc : cuc;
+  __half* o = out + idx * Cpad;
+  for (int c0 = 0; c0 < Cpad; c0 += 8) {
+    Half8 v;
+#pragma unroll
+    for (int e = 0; e < 8; e += 2) {
+      float a[2];
+#pragma unroll
+      for (int u = 0; u < 2; u++) {
+        const int c = c0 + e + u;
+        float val = 0.f;
+        if (c < Cx) {
+          const long long xi = ((long long)f * Cx + c) * HW + pix;
+          float xv = x[xi];
+          if (eps) {
+            xv = xv + (eps[xi] * s_noise) * churn;
+            if (n == f) x_hat_out[xi] = xv;
+          }
+          val = xv * c_in;
+        } else if (c < Cx + Cc && cat != nullptr) {
+          val = (float)cat[((long long)f * Cc + (c - Cx)) * HW + pix];
+        }
+        a[u] = val;
+      }
+      v.h[e / 2] = __floats2half2_rn(a[0], a[1]);
+    }
+    *reinterpret_cast<Half8*>(o + c0) = v;
+  }
+}
+
+// The post step with an ancestral update and an optional guider: scale == nullptr reads F network rows (IdentityGuider), else
+// 2F rows combined with scale[f % T].  x_out = x + d (sigma_to - sigma), then + (eps * s_noise) * sigma_up where sigma_next > 0
+// (AncestralSampler, sampling.py:158-170).
+__global__ void sampler_post_ancestral_kernel(const __half* __restrict__ net, int net_ld, const float* __restrict__ x,
+                                              const float* __restrict__ sigma, const float* __restrict__ sigma_to,
+                                              const float* __restrict__ scale, int T, const float* __restrict__ eps,
+                                              float s_noise, const float* __restrict__ sigma_up,
+                                              const float* __restrict__ sigma_next, int F, int Cx, int HW,
+                                              float* __restrict__ x_out, float* __restrict__ den_out) {
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (long long)F * HW) return;
+  const int f = (int)(idx / HW), pix = (int)(idx - (long long)f * HW);
+  const float sg = sigma[f], st = sigma_to[f];
+  const float d2 = sg * sg + 1.f;
+  const float c_skip = 1.f / d2, c_out = -sg * rsqrtf(d2);
+  const bool noise = eps != nullptr && sigma_next[f] > 0.f;
+  const float su = eps != nullptr ? sigma_up[f] : 0.f;
+  const __half* nc = net + ((long long)((scale ? F : 0) + f) * HW + pix) * net_ld;
+  const __half* nu = net + ((long long)f * HW + pix) * net_ld;
+  const float gs = scale ? scale[f % T] : 1.f;
+  for (int c = 0; c < Cx; c++) {
+    const long long xi = ((long long)f * Cx + c) * HW + pix;
+    const float xv = x[xi];
+    float den = __half2float(nc[c]) * c_out + xv * c_skip;
+    if (scale) {
+      const float du = __half2float(nu[c]) * c_out + xv * c_skip;
+      den = du + gs * (den - du);
+    }
+    if (den_out) den_out[xi] = den;
+    const float d = (xv - den) / sg;
+    float xn = xv + d * (st - sg);
+    if (noise) xn = xn + (eps[xi] * s_noise) * su;
+    x_out[xi] = xn;
+  }
+}
+
+struct LincombTerms {
+  const float* x[8];
+  const float* c[8];
+};
+
+// out = sum_k c_k[f] x_k over up to 8 terms: linear multistep of order 4 over (x, D) pairs, DPM-Solver++(2S)'s selected update.
+__global__ void lincomb_kernel(float* __restrict__ out, LincombTerms t, int nterms, int per_sample, long long n) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int f = (int)(i / per_sample);
+  float v = t.c[0][f] * t.x[0][i];
+#pragma unroll
+  for (int k = 1; k < 8; k++)
+    if (k < nterms) v += t.c[k][f] * t.x[k][i];
+  out[i] = v;
+}
+
 // out = c0 x0 + c1 x1 + c2 x2 + c3 x3 with per-sample fp32 coefficients: the solver algebra of the multi-evaluation samplers
 // (Heun's trapezoid update, DPM-Solver++(2M)'s extrapolated update) on the fp32 sampler state, one launch.
 __global__ void lincomb4_kernel(float* __restrict__ out, const float* __restrict__ x0, const float* __restrict__ x1,
@@ -246,6 +351,64 @@ extern "C" int hi3d_sampler_lincomb4(float* out, const float* x0, const float* x
   lincomb4_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(out, x0, x1, x2, x3, c0, c1, c2, c3,
                                                                                 (int)per_sample, n);
   return check_launch("hi3d_sampler_lincomb4");
+}
+
+extern "C" int hi3d_sampler_pre_ex(const float* x, const float* sigma, const float* sigma_from, const float* eps,
+                                   float s_noise, const void* concat_uc, const void* concat_c, int concat_is_fp32, int guided,
+                                   int F, int Cx, int Cc, int H, int W, int Cpad, void* out, float* c_noise_out,
+                                   float* x_hat_out, void* stream) {
+  if (!x || !sigma || !out || F <= 0 || Cx <= 0 || Cc < 0 || H <= 0 || W <= 0 || (Cpad % 8) || Cpad < Cx + Cc ||
+      ((uintptr_t)out & 15) || (Cc > 0 && !concat_c) || (guided != 0 && guided != 1) ||
+      (eps && (!sigma_from || !x_hat_out))) {
+    set_error("hi3d_sampler_pre_ex: bad arguments (F=%d Cx=%d Cc=%d Cpad=%d guided=%d)", F, Cx, Cc, Cpad, guided);
+    return -2;
+  }
+  const int rows = guided ? 2 : 1;
+  const long long total = (long long)rows * F * H * W;
+  const unsigned blocks = (unsigned)((total + 255) / 256);
+  if (concat_is_fp32)
+    sampler_pre_ex_kernel<float><<<blocks, 256, 0, (cudaStream_t)stream>>>(
+        x, sigma, sigma_from, eps, s_noise, (const float*)concat_uc, (const float*)concat_c, rows, F, Cx, Cc, H * W, Cpad,
+        (__half*)out, c_noise_out, x_hat_out);
+  else
+    sampler_pre_ex_kernel<__half><<<blocks, 256, 0, (cudaStream_t)stream>>>(
+        x, sigma, sigma_from, eps, s_noise, (const __half*)concat_uc, (const __half*)concat_c, rows, F, Cx, Cc, H * W, Cpad,
+        (__half*)out, c_noise_out, x_hat_out);
+  return check_launch("hi3d_sampler_pre_ex");
+}
+
+extern "C" int hi3d_sampler_post_ancestral(const void* net, int net_ld, const float* x, const float* sigma,
+                                           const float* sigma_to, const float* scale, int T, const float* eps, float s_noise,
+                                           const float* sigma_up, const float* sigma_next, int F, int Cx, int H, int W,
+                                           float* x_out, float* denoised_out, void* stream) {
+  if (!net || !x || !sigma || !sigma_to || !x_out || F <= 0 || Cx <= 0 || H <= 0 || W <= 0 || net_ld < Cx ||
+      (scale && T <= 0) || (eps && (!sigma_up || !sigma_next))) {
+    set_error("hi3d_sampler_post_ancestral: bad arguments (F=%d Cx=%d net_ld=%d T=%d)", F, Cx, net_ld, T);
+    return -2;
+  }
+  const long long total = (long long)F * H * W;
+  sampler_post_ancestral_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+      (const __half*)net, net_ld, x, sigma, sigma_to, scale, T, eps, s_noise, sigma_up, sigma_next, F, Cx, H * W, x_out,
+      denoised_out);
+  return check_launch("hi3d_sampler_post_ancestral");
+}
+
+extern "C" int hi3d_sampler_lincomb(float* out, const float* const* xs, const float* const* cs, int nterms, int F,
+                                    int64_t per_sample, void* stream) {
+  bool ok = out && xs && cs && nterms >= 1 && nterms <= 8 && F > 0 && per_sample > 0 && per_sample <= 2147483647LL;
+  LincombTerms t = {};
+  for (int k = 0; ok && k < nterms; k++) {
+    ok = xs[k] && cs[k];
+    t.x[k] = xs[k];
+    t.c[k] = cs[k];
+  }
+  if (!ok) {
+    set_error("hi3d_sampler_lincomb: bad arguments (nterms=%d F=%d)", nterms, F);
+    return -2;
+  }
+  const long long n = (long long)F * per_sample;
+  lincomb_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(out, t, nterms, (int)per_sample, n);
+  return check_launch("hi3d_sampler_lincomb");
 }
 
 extern "C" int hi3d_renoise_blend(float* lat, const float* init, const float* z, float alpha, float sigma, int64_t n,

@@ -165,14 +165,19 @@ class VideoLDM(DiffusionEngine):
 
     # ---- hot loop of pipeline_i2v_eval_v01.py:62-98 (after conditioning) ------------------------------------------------------
     @torch.no_grad()
-    def sample_stage1(self, c: Dict, uc: Dict, randn: torch.Tensor, decode: bool = True, shard=None):
+    def sample_stage1(self, c: Dict, uc: Dict, randn: torch.Tensor, decode: bool = True, shard=None, generators=None):
         """randn: (B * T, 4, h, w) for B objects; c / uc: crossattn (B, 1, 1024), vector (B, 768), concat (B * T, 4, h, w).
         Returns B * T latents or decoded frames, object-major; object i's frames are what a run over object i alone gives.
         shard = (rank, world): `randn` and c/uc['concat'] hold only this rank's frames (frame-sharded video); the
-        returned latents / decoded frames are this rank's frames too."""
+        returned latents / decoded frames are this rank's frames too.  generators: one CUDA generator per object for the
+        stochastic samplers' per-step noise (None: the global one)."""
         T = self.num_samples
         den = self.bind_denoiser(shard=shard, image_only_indicator=None, num_video_frames=T)
-        samples = self.sampler(den, randn, cond=c, uc=uc)
+        self.sampler.noise_generators = generators
+        try:
+            samples = self.sampler(den, randn, cond=c, uc=uc)
+        finally:
+            self.sampler.noise_generators = None
         if not decode:
             return samples
         return self.decode_first_stage(samples.half())
@@ -207,10 +212,11 @@ class VideoLDMStage2(VideoLDM):
     # ---- hot loop of pipeline_i2v_eval_v02.py:86-137 ---------------------------------------------------------------------------
     @torch.no_grad()
     def sample_stage2(self, c: Dict, uc: Dict, init_latents: torch.Tensor, z: torch.Tensor, decode: bool = True,
-                      alpha_pow: float = 40.0, shard=None):
+                      alpha_pow: float = 40.0, shard=None, generators=None):
         """init_latents ~ N(0,1) (B*T,4,h,w) fp32; z = encode_first_stage(low-res frames) (B*T,4,h,w), B objects
         object-major as in sample_stage1; returns B * T latents or decoded frames.
-        shard = (rank, world): all per-frame tensors hold only this rank's frames."""
+        shard = (rank, world): all per-frame tensors hold only this rank's frames.  generators: as in sample_stage1 (the
+        churn noise of --s_churn)."""
         from . import ops
         smp = self.sampler
         T = self.num_samples
@@ -222,10 +228,14 @@ class VideoLDMStage2(VideoLDM):
         init_latents = init_latents.float().contiguous()
         z = z.float().contiguous()
         den = self.bind_denoiser(shard=shard, image_only_indicator=None, num_video_frames=T)
-        for i in smp.get_sigma_gen(num_sigmas):
-            alpha = math.pow(0.5 * (1 + math.cos(i * 1.0 / smp.num_steps)), alpha_pow)
-            ops.renoise_blend(latents, init_latents, z, alpha, sig_host[i])           # v02:131-132
-            latents = smp.step_call(den, latents, i, s_in, sigmas, num_sigmas, c, uc)   # v02:134-135
+        smp.noise_generators = generators
+        try:
+            for i in smp.get_sigma_gen(num_sigmas):
+                alpha = math.pow(0.5 * (1 + math.cos(i * 1.0 / smp.num_steps)), alpha_pow)
+                ops.renoise_blend(latents, init_latents, z, alpha, sig_host[i])           # v02:131-132
+                latents = smp.step_call(den, latents, i, s_in, sigmas, num_sigmas, c, uc)   # v02:134-135
+        finally:
+            smp.noise_generators = None
         if not decode:
             return latents
         return self.decode_first_stage(latents.half())

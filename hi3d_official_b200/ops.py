@@ -408,6 +408,68 @@ def sampler_lincomb(out: torch.Tensor, terms):
     return out
 
 
+def sampler_pre_ex(x: torch.Tensor, sigma: torch.Tensor, concat_uc: Optional[torch.Tensor], concat_c: Optional[torch.Tensor],
+                   out: torch.Tensor, guided: bool, c_noise_out: Optional[torch.Tensor] = None,
+                   churn: Optional[Tuple[torch.Tensor, torch.Tensor, float, torch.Tensor]] = None):
+    """hi3d_sampler_pre_ex; churn = (sigma_from, eps, s_noise, x_hat_out)."""
+    _chk32(x, "x"); _chk32(sigma, "sigma"); _chk16(out, "out")
+    F_, Cx, H, W = x.shape
+    Cc, is32 = 0, 0
+    if concat_c is not None:
+        Cc = concat_c.shape[1]
+        is32 = int(concat_c.dtype == torch.float32)
+        for t in (concat_c, concat_uc):
+            if t is not None and (not t.is_contiguous() or t.dtype != concat_c.dtype or tuple(t.shape) != (F_, Cc, H, W)):
+                raise ValueError("concat tensors must be contiguous NCHW of identical dtype/shape [F, Cc, H, W]")
+    sigma_from = eps = x_hat = None
+    s_noise = 0.0
+    if churn is not None:
+        sigma_from, eps, s_noise, x_hat = churn
+        _chk32(sigma_from, "sigma_from"); _chk32(eps, "eps"); _chk32(x_hat, "x_hat_out")
+        if eps.shape != x.shape or x_hat.shape != x.shape:
+            raise ValueError("eps / x_hat_out must have the shape of x")
+    N.check(N.load().hi3d_sampler_pre_ex(x.data_ptr(), sigma.data_ptr(), _ptr(sigma_from), _ptr(eps), float(s_noise),
+                                         _ptr(concat_uc), _ptr(concat_c), is32, int(guided), F_, Cx, Cc, H, W, out.shape[-1],
+                                         out.data_ptr(), _ptr(c_noise_out), _ptr(x_hat), _stream()), "hi3d_sampler_pre_ex")
+
+
+def sampler_post_ancestral(net: torch.Tensor, x: torch.Tensor, sigma: torch.Tensor, sigma_to: torch.Tensor,
+                           scale: Optional[torch.Tensor], x_out: torch.Tensor, denoised_out: Optional[torch.Tensor] = None,
+                           noise: Optional[Tuple[torch.Tensor, float, torch.Tensor, torch.Tensor]] = None):
+    """hi3d_sampler_post_ancestral; scale None = IdentityGuider (F network rows); noise = (eps, s_noise, sigma_up, sigma_next)."""
+    _chk16(net, "net"); _chk32(x, "x"); _chk32(sigma, "sigma"); _chk32(sigma_to, "sigma_to"); _chk32(x_out, "x_out")
+    F_, Cx, H, W = x.shape
+    if scale is not None:
+        _chk32(scale, "scale")
+    eps, s_noise, sigma_up, sigma_next = noise if noise is not None else (None, 0.0, None, None)
+    if noise is not None:
+        _chk32(eps, "eps"); _chk32(sigma_up, "sigma_up"); _chk32(sigma_next, "sigma_next")
+        if eps.shape != x.shape:
+            raise ValueError("eps must have the shape of x")
+    N.check(N.load().hi3d_sampler_post_ancestral(net.data_ptr(), net.shape[-1], x.data_ptr(), sigma.data_ptr(),
+                                                 sigma_to.data_ptr(), _ptr(scale), 0 if scale is None else scale.numel(),
+                                                 _ptr(eps), float(s_noise), _ptr(sigma_up), _ptr(sigma_next), F_, Cx, H, W,
+                                                 x_out.data_ptr(), _ptr(denoised_out), _stream()),
+            "hi3d_sampler_post_ancestral")
+
+
+def sampler_lincomb8(out: torch.Tensor, terms):
+    """out = sum_k c_k[f] * x_k; terms = [(x_k fp32 [F, ...], c_k fp32 [F]), ...] (1..8 terms): hi3d_sampler_lincomb."""
+    if not 1 <= len(terms) <= 8:
+        raise ValueError("1..8 terms")
+    _chk32(out, "out")
+    F_ = out.shape[0]
+    for x, c in terms:
+        _chk32(x, "x"); _chk32(c, "c")
+        if x.shape != out.shape or c.numel() != F_:
+            raise ValueError("lincomb: shape mismatch")
+    xs = (C.c_void_p * len(terms))(*[x.data_ptr() for x, _ in terms])
+    cs = (C.c_void_p * len(terms))(*[c.data_ptr() for _, c in terms])
+    N.check(N.load().hi3d_sampler_lincomb(out.data_ptr(), xs, cs, len(terms), F_, out.numel() // F_, _stream()),
+            "hi3d_sampler_lincomb")
+    return out
+
+
 def renoise_blend(lat: torch.Tensor, init: torch.Tensor, z: torch.Tensor, alpha: float, sigma: float):
     _chk32(lat, "lat"); _chk32(init, "init"); _chk32(z, "z")
     N.check(N.load().hi3d_renoise_blend(lat.data_ptr(), init.data_ptr(), z.data_ptr(), alpha, sigma, lat.numel(),

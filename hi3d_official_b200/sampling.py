@@ -6,13 +6,16 @@
   IdentityWrapper / OpenAIWrapper   wrappers.py:8-34
   IdentityGuider / VanillaCFG / LinearPredictionGuider   guiders.py:24-99
   BaseDiffusionSampler / EDMSampler / EulerEDMSampler (+ Hi3D's step_call)   sampling.py:21-147,228-232
+  HeunEDMSampler / DPMPP2MSampler   sampling.py:235-254,304-379
+  AncestralSampler / EulerAncestralSampler / DPMPP2SAncestralSampler / LinearMultistepSampler   sampling.py:150-226,254-302
 
 Two execution paths with identical results:
   * generic: `denoiser` is any Python callable (x, sigma, cond) -> denoised, exactly like the reference; the
     few elementwise ops on the (16, 4, h, w) fp32 sampler state are torch glue around whatever the callable does;
   * fused (the product path): when the callable is a `FusedDenoiser` binding (Denoiser + OpenAIWrapper(VideoUNet)),
     one Euler step is  hi3d_sampler_pre -> VideoUNet launch plan -> hi3d_sampler_post  with no host sync,
-    no torch math and the step-invariant conditioning computed once per video.
+    no torch math and the step-invariant conditioning computed once per video.  Every sampler and guider takes it: each
+    network evaluation is a CUDA-graph replay, and a stochastic step's noise is drawn into a static buffer before the replay.
 """
 from __future__ import annotations
 
@@ -211,41 +214,48 @@ class FusedDenoiser:
 
 
 class _FusedState:
-    """Per-(shape) fused step executor bound to one VideoUNet launch plan."""
+    """Per-(shape, guider) fused network evaluation bound to one VideoUNet launch plan.  `scale` is the guider's CFG scale per
+    frame ([T] for LinearPredictionGuider, [1] for VanillaCFG) or None for IdentityGuider, whose plan holds F rows (the
+    conditional half only) instead of 2F."""
 
-    def __init__(self, unet: VideoUNet, F_: int, H: int, W: int, T: int, scale: torch.Tensor, shard=None):
-        self.plan = unet.get_plan(2 * F_, H, W, T, shard=shard)
+    def __init__(self, unet: VideoUNet, F_: int, H: int, W: int, T: int, scale: Optional[torch.Tensor], shard=None):
+        self.guided = scale is not None
+        self.plan = unet.get_plan((2 if self.guided else 1) * F_, H, W, T, shard=shard)
         dev = unet.device
-        self.scale = scale.reshape(-1).to(device=dev, dtype=torch.float32).contiguous()
+        self.scale = None if scale is None else scale.reshape(-1).to(device=dev, dtype=torch.float32).contiguous()
         self.key = None
         self.cc = self.cuc = None
-        # CUDA-graph replay of the whole step (pre -> ~750 launches -> post): static I/O buffers + one graph.  Frame-sharded
-        # plans are captured too when their exchanges are peer-memory kernels (every rank replays the same graph, the flag
-        # barriers inside it keep the ranks in step); with NCCL exchanges the step stays eager.
+        # CUDA-graph replay of every kind of evaluation (pre -> ~750 launches -> post), one graph per kind, all reading and
+        # writing the static buffers below.  Frame-sharded plans are captured too when their exchanges are peer-memory
+        # kernels (every rank replays the same graph, the flag barriers inside it keep the ranks in step); with NCCL
+        # exchanges the evaluations stay eager.
         self.use_graph = os.environ.get("HI3D_CUDA_GRAPH", "1") != "0" and (shard is None or self.plan.exchange_mode == "peer")
-        self._graph = None
-        self._gx = torch.zeros(F_, 4, H, W, dtype=torch.float32, device=dev)
-        self._gxo = torch.zeros_like(self._gx)
-        self._gs = torch.ones(F_, dtype=torch.float32, device=dev)
-        self._gsn = torch.ones(F_, dtype=torch.float32, device=dev)
+        self._graphs: Dict[tuple, Tuple[torch.cuda.CUDAGraph, int]] = {}
+        self._gx, self._gxo, self._gden, self._gxh, self._geps = (torch.zeros(F_, 4, H, W, dtype=torch.float32, device=dev)
+                                                                  for _ in range(5))
+        self._gs, self._gst, self._gsf, self._gsu, self._gsn = (torch.ones(F_, dtype=torch.float32, device=dev)
+                                                                for _ in range(5))
 
     def set_conditioning(self, c: dict, uc: dict):
-        ctx = torch.cat((uc["crossattn"], c["crossattn"]), 0)
-        y = torch.cat((uc["vector"], c["vector"]), 0)
+        if self.guided:
+            ctx = torch.cat((uc["crossattn"], c["crossattn"]), 0)
+            y = torch.cat((uc["vector"], c["vector"]), 0)
+        else:                                   # IdentityGuider.prepare_inputs: the conditional rows alone
+            ctx, y = c["crossattn"], c["vector"]
         self.plan.prepare_conditioning(ctx, y)
         cc, cuc = c.get("concat", None), uc.get("concat", None)
         if cc is None:
             if self.cc is not None:
-                self._graph = None
+                self._graphs.clear()
             self.cc = self.cuc = None
             return
         dt = cc.dtype if cc.dtype in (torch.float16, torch.float32) else torch.float32
         if self.cc is None or self.cc.shape != cc.shape or self.cc.dtype != dt:
-            # persistent copies: their addresses are baked into the captured graph
+            # persistent copies: their addresses are baked into the captured graphs
             self.cc, self.cuc = torch.empty_like(cc, dtype=dt).contiguous(), torch.empty_like(cc, dtype=dt).contiguous()
-            self._graph = None
+            self._graphs.clear()
         self.cc.copy_(cc)
-        if cuc is None:
+        if cuc is None or not self.guided:
             self.cuc.zero_()
         else:
             self.cuc.copy_(cuc)
@@ -255,55 +265,86 @@ class _FusedState:
         return tuple((k, d[k].data_ptr(), d[k]._version, tuple(d[k].shape)) for d in (c, uc) for k in sorted(d)
                      if torch.is_tensor(d[k]))
 
-    def _launch(self, x, sigma, next_sigma, x_out, den):
+    def noise_buffer(self) -> Optional[torch.Tensor]:
+        """Where a sampler draws the step's noise before a replay (the graphs read it from there), or None when eager."""
+        return self._geps if self.use_graph else None
+
+    def _launch(self, x, sigma, sigma_to, x_out, den, churn=None, noise=None):
+        """pre -> launch plan -> post.  churn = (sigma_from, eps, s_noise, x_hat): the network sees the churned x_hat at sigma
+        and the update starts from it.  noise = (eps, s_noise, sigma_up, sigma_next): the ancestral noise of the update.
+        The CFG-guided Euler evaluation keeps hi3d_sampler_pre / hi3d_sampler_post."""
         plan = self.plan
         F_, Cx, H, W = x.shape
-        ops.sampler_pre(x, sigma, self.cuc, self.cc, plan.xin.t.view(2 * F_, H, W, CIN_PAD), c_noise_out=plan.t_in)
+        xin = plan.xin.t.view(-1, H, W, CIN_PAD)
+        if self.guided and churn is None:
+            ops.sampler_pre(x, sigma, self.cuc, self.cc, xin, c_noise_out=plan.t_in)
+        else:
+            ops.sampler_pre_ex(x, sigma, self.cuc, self.cc, xin, self.guided, c_noise_out=plan.t_in, churn=churn)
         plan.run()
-        ops.sampler_post(plan.net_out.t, x, sigma, next_sigma, self.scale, x_out, den)
+        xp = x if churn is None else churn[3]
+        if self.guided and noise is None:
+            ops.sampler_post(plan.net_out.t, xp, sigma, sigma_to, self.scale, x_out, den)
+        else:
+            ops.sampler_post_ancestral(plan.net_out.t, xp, sigma, sigma_to, self.scale, x_out, den, noise)
 
-    def denoise(self, x: torch.Tensor, sigma: torch.Tensor) -> torch.Tensor:
-        """Guided denoised latents D(x, sigma) on the fused path (sampler_pre -> launch plan -> sampler_post): the network
-        evaluation of ANY sampler (Heun's second evaluation, DPM-Solver++), without the Euler update."""
-        plan = self.plan
-        x = x.contiguous()
-        sigma = sigma.contiguous()
-        F_, Cx, H, W = x.shape
-        ops.sampler_pre(x, sigma, self.cuc, self.cc, plan.xin.t.view(2 * F_, H, W, CIN_PAD), c_noise_out=plan.t_in)
-        plan.run()
-        den = torch.empty_like(x)
-        if getattr(self, "_scratch", None) is None or self._scratch.shape != x.shape:
-            self._scratch = torch.empty_like(x)
-        ops.sampler_post(plan.net_out.t, x, sigma, sigma, self.scale, self._scratch, den)
-        return den
-
-    def step(self, x: torch.Tensor, sigma: torch.Tensor, next_sigma: torch.Tensor, want_denoised: bool = False):
-        if self.use_graph and not want_denoised and x.shape == self._gx.shape:
+    def run(self, x: torch.Tensor, sigma: torch.Tensor, sigma_to: torch.Tensor, want_denoised: bool = False,
+            churn: Optional[tuple] = None, noise: Optional[tuple] = None):
+        """One network evaluation and its update x + (x - D)/sigma * (sigma_to - sigma): returns (x_out, D or None, x_hat or
+        None).  churn = (sigma_from, eps, s_noise) and noise = (eps, s_noise, sigma_up, sigma_next) as in `_launch`.  With
+        graphs on, the inputs are copied into the static buffers (eps is drawn there directly when it is `noise_buffer()`)
+        and the graph of this kind of call is replayed; it is captured on first use."""
+        if self.use_graph and x.shape == self._gx.shape:
+            key = (want_denoised, None if churn is None else float(churn[2]), None if noise is None else float(noise[1]))
             self._gx.copy_(x)
             self._gs.copy_(sigma)
-            self._gsn.copy_(next_sigma)
-            if self._graph is None:
-                self._launch(self._gx, self._gs, self._gsn, self._gxo, None)        # eager warm-up (lazy one-time init)
+            self._gst.copy_(sigma_to)
+            eps = churn[1] if churn is not None else noise[0] if noise is not None else None
+            if eps is not None and eps.data_ptr() != self._geps.data_ptr():
+                self._geps.copy_(eps)
+            g_churn = g_noise = None
+            if churn is not None:
+                self._gsf.copy_(churn[0])
+                g_churn = (self._gsf, self._geps, float(churn[2]), self._gxh)
+            if noise is not None:
+                self._gsu.copy_(noise[2])
+                self._gsn.copy_(noise[3])
+                g_noise = (self._geps, float(noise[1]), self._gsu, self._gsn)
+            args = (self._gx, self._gs, self._gst, self._gxo, self._gden if want_denoised else None, g_churn, g_noise)
+            if key not in self._graphs:
+                self._launch(*args)                  # eager warm-up (lazy one-time init)
                 torch.cuda.synchronize()
                 g = torch.cuda.CUDAGraph()
                 n0 = _native.launch_count()
                 with torch.cuda.graph(g):
-                    self._launch(self._gx, self._gs, self._gsn, self._gxo, None)
-                self._graph_launches = _native.launch_count() - n0
-                _native.note_graph_replay(-self._graph_launches)      # capture-time calls did not execute
-                self._graph = g
-            self._graph.replay()
-            _native.note_graph_replay(self._graph_launches)
-            return self._gxo.clone()
-        plan = self.plan
+                    self._launch(*args)
+                n = _native.launch_count() - n0
+                _native.note_graph_replay(-n)        # capture-time calls did not execute
+                self._graphs[key] = (g, n)
+            g, n = self._graphs[key]
+            g.replay()
+            _native.note_graph_replay(n)
+            return (self._gxo.clone(), self._gden.clone() if want_denoised else None,
+                    self._gxh.clone() if churn is not None else None)
         x = x.contiguous()
-        sigma, next_sigma = sigma.contiguous(), next_sigma.contiguous()
-        F_, Cx, H, W = x.shape
-        ops.sampler_pre(x, sigma, self.cuc, self.cc, plan.xin.t.view(2 * F_, H, W, CIN_PAD), c_noise_out=plan.t_in)
-        plan.run()
         x_out = torch.empty_like(x)
         den = torch.empty_like(x) if want_denoised else None
-        ops.sampler_post(plan.net_out.t, x, sigma, next_sigma, self.scale, x_out, den)
+        x_hat = None
+        if churn is not None:
+            x_hat = torch.empty_like(x)
+            churn = (churn[0].contiguous(), churn[1].contiguous(), churn[2], x_hat)
+        if noise is not None:
+            noise = (noise[0].contiguous(), noise[1], noise[2].contiguous(), noise[3].contiguous())
+        self._launch(x, sigma.contiguous(), sigma_to.contiguous(), x_out, den, churn, noise)
+        return x_out, den, x_hat
+
+    def denoise(self, x: torch.Tensor, sigma: torch.Tensor, churn: Optional[tuple] = None):
+        """Guided denoised latents D(x, sigma) on the fused path: the network evaluation of ANY sampler (Heun's second
+        evaluation, DPM-Solver++), without the update.  With churn = (sigma_from, eps, s_noise) returns (D, x_hat)."""
+        _, den, x_hat = self.run(x, sigma, sigma, True, churn)
+        return den if churn is None else (den, x_hat)
+
+    def step(self, x: torch.Tensor, sigma: torch.Tensor, next_sigma: torch.Tensor, want_denoised: bool = False):
+        x_out, den, _ = self.run(x, sigma, next_sigma, want_denoised)
         return (x_out, den) if want_denoised else x_out
 
 
@@ -322,6 +363,24 @@ class BaseDiffusionSampler:
         self.verbose = verbose
         self.device = device
         self._fused: Dict[tuple, _FusedState] = {}
+        self.noise_sampler = lambda x: torch.randn_like(x)
+        # one generator per object (frames object-major): each stochastic step draws object i's noise from generator i, so an
+        # object's result does not depend on the batch it is sampled in.  None: `noise_sampler`, i.e. the global generator.
+        self.noise_generators: Optional[List[torch.Generator]] = None
+
+    def draw_noise(self, x: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """This step's eps ~ N(0, 1) in the shape of x, written to `out` when given."""
+        gens = self.noise_generators
+        if not gens:
+            e = self.noise_sampler(x)
+            return e if out is None else out.copy_(e)
+        if x.shape[0] % len(gens):
+            raise ValueError(f"{x.shape[0]} frames cannot be split over {len(gens)} objects")
+        out = torch.empty_like(x) if out is None else out
+        n = x.shape[0] // len(gens)
+        for i, g in enumerate(gens):
+            out[i * n:(i + 1) * n].normal_(generator=g)
+        return out
 
     def prepare_sampling_loop(self, x, cond, uc=None, num_steps=None):
         sigmas = self.discretization(self.num_steps if num_steps is None else num_steps, device=self.device)
@@ -344,16 +403,28 @@ class BaseDiffusionSampler:
         return self.guider(denoised, sigma)
 
     # -- fused path (shared by every sampler) -------------------------------------------------------------------
+    frame_sharded = False        # whether the sampler runs frame-sharded plans (those that ran them before the other samplers)
+
     def _fused_state(self, denoiser, x, cond, uc, refresh: bool) -> Optional[_FusedState]:
-        if not (isinstance(denoiser, FusedDenoiser) and denoiser.fusable()
-                and isinstance(self.guider, LinearPredictionGuider) and x.is_cuda and x.dtype == torch.float32):
+        if not (isinstance(denoiser, FusedDenoiser) and denoiser.fusable() and x.is_cuda and x.dtype == torch.float32):
             return None
         unet = denoiser.network.diffusion_model
         T = int(denoiser.kwargs["num_video_frames"])
-        if T != self.guider.num_frames:
-            return None
         shard = denoiser.shard
-        scale = self.guider.scale.reshape(-1)
+        g = self.guider
+        if shard is not None and not (self.frame_sharded and isinstance(g, LinearPredictionGuider)):
+            raise NotImplementedError(f"frame-sharded sampling runs EulerEDMSampler, HeunEDMSampler and DPMPP2MSampler with "
+                                      f"LinearPredictionGuider; got {type(self).__name__} with {type(g).__name__}")
+        if isinstance(g, LinearPredictionGuider):
+            if T != g.num_frames:
+                return None
+            scale = g.scale.reshape(-1)
+        elif isinstance(g, VanillaCFG):
+            scale = torch.tensor([float(g.scale)])
+        elif isinstance(g, IdentityGuider):
+            scale = None
+        else:
+            return None
         if shard is not None:             # this rank holds frames [rank*Tl, (rank+1)*Tl) of every clip
             if T % shard[1]:
                 raise ValueError(f"{T} frames cannot be sharded over {shard[1]} ranks")
@@ -363,8 +434,9 @@ class BaseDiffusionSampler:
         if x.shape[0] % T:
             return None
         F_, _, H, W = x.shape
-        key = (id(unet), F_, H, W, T, unet.engine, shard)
-        pkey = (2 * F_, H, W, T, unet.engine) if shard is None else (2 * F_, H, W, T, unet.engine, shard)
+        rows = F_ if scale is None else 2 * F_
+        key = (id(unet), F_, H, W, T, unet.engine, shard, rows)
+        pkey = (rows, H, W, T, unet.engine) if shard is None else (rows, H, W, T, unet.engine, shard)
         st = self._fused.get(key)
         if st is None or st.plan is not unet._plans.get(pkey):
             st = self._fused[key] = _FusedState(unet, F_, H, W, T, scale, shard)
@@ -373,7 +445,6 @@ class BaseDiffusionSampler:
             st.set_conditioning(cond, uc)
             st.key = ck
         return st
-
 
     def get_sigma_gen(self, num_sigmas):
         sigma_generator = range(num_sigmas - 1)
@@ -396,6 +467,8 @@ class SingleStepDiffusionSampler(BaseDiffusionSampler):
 
 
 class EDMSampler(SingleStepDiffusionSampler):
+    frame_sharded = True
+
     def __init__(self, s_churn=0.0, s_tmin=0.0, s_tmax=float("inf"), s_noise=1.0, *args, **kwargs):
         super().__init__(*args, **kwargs)
         self.s_churn, self.s_tmin, self.s_tmax, self.s_noise = s_churn, s_tmin, s_tmax, s_noise
@@ -409,15 +482,22 @@ class EDMSampler(SingleStepDiffusionSampler):
         return euler_step
 
     def sampler_step(self, sigma, next_sigma, denoiser, x, cond, uc=None, gamma=0.0, _refresh=False):
-        if gamma == 0:
-            st = self._fused_state(denoiser, x, cond, default(uc, cond), _refresh)
-            if st is not None and type(self).possible_correction_step is EDMSampler.possible_correction_step:
-                return st.step(x, sigma, next_sigma)
-        sigma_hat = sigma * (gamma + 1.0)
+        st = self._fused_state(denoiser, x, cond, default(uc, cond), _refresh)
+        sigma_hat = sigma if gamma == 0 else sigma * (gamma + 1.0)
+        churn = None
         if gamma > 0:
-            eps = torch.randn_like(x) * self.s_noise
-            x = x + eps * append_dims(sigma_hat ** 2 - sigma ** 2, x.ndim) ** 0.5
-        denoised = self.denoise(x, denoiser, sigma_hat, cond, uc)
+            if st is not None and denoiser.shard is None:
+                # x_hat = x + s_noise sqrt(sigma_hat^2 - sigma^2) eps inside the pre kernel, eps drawn before the replay
+                churn = (sigma, self.draw_noise(x, st.noise_buffer()), self.s_noise)
+            else:
+                eps = self.draw_noise(x) * self.s_noise
+                x = x + eps * append_dims(sigma_hat ** 2 - sigma ** 2, x.ndim) ** 0.5
+        if st is not None and type(self).possible_correction_step is EDMSampler.possible_correction_step:
+            return st.run(x, sigma_hat, next_sigma, churn=churn)[0]
+        if churn is not None:
+            denoised, x = st.denoise(x, sigma_hat, churn)
+        else:
+            denoised = self.denoise(x, denoiser, sigma_hat, cond, uc)
         d = (x - denoised) / append_dims(sigma_hat, x.ndim)            # to_d, sampling_utils.py:34
         dt = append_dims(next_sigma - sigma_hat, x.ndim)
         self._heun_ctx = (next_sigma - sigma_hat).float().contiguous() if x.is_cuda else None
@@ -475,6 +555,7 @@ class HeunEDMSampler(EDMSampler):
 class DPMPP2MSampler(BaseDiffusionSampler):
     """sampling.py:305-379 (DPM-Solver++(2M), Lu et al. 2022) in t = -log(sigma): one evaluation per step; from the
     second step on the denoised estimate is extrapolated with the previous one (ratio r of the two log-step sizes)."""
+    frame_sharded = True
 
     @staticmethod
     def _t(sigma):                       # sampling_utils.py: to_neg_log_sigma
@@ -514,3 +595,216 @@ class DPMPP2MSampler(BaseDiffusionSampler):
             x, prev_d = self.sampler_step(prev_d, None if i == 0 else s_in * sigmas[i - 1], s_in * sigmas[i],
                                           s_in * sigmas[i + 1], denoiser, x, cond, uc=uc)
         return x
+
+
+# ------------------------------------------------------------------------------------------------------------
+# The ancestral and linear multistep samplers of the sgm surface (sampling.py:150-226, 254-302).  On the fused path every network
+# evaluation is a graph replay; the Euler ancestral step is ONE replay (hi3d_sampler_post_ancestral adds the noise), and the
+# solver algebra of DPM-Solver++(2S) and LMS is one hi3d_sampler_lincomb launch per update.
+# ------------------------------------------------------------------------------------------------------------
+def ancestral_sigmas(sigma_from: torch.Tensor, sigma_to: torch.Tensor, eta: float = 1.0):
+    """The ancestral split of a step from sigma_from to sigma_to (Karras et al. 2022, k-diffusion): the deterministic part goes
+    to sigma_down, and fresh noise of standard deviation sigma_up brings it back to sigma_to (sigma_down^2 + sigma_up^2 =
+    sigma_to^2).  eta = 0 gives the deterministic step."""
+    if not eta:
+        return sigma_to, torch.zeros_like(sigma_to)
+    up = (sigma_to ** 2 * (sigma_from ** 2 - sigma_to ** 2) / sigma_from ** 2) ** 0.5 * eta
+    sigma_up = torch.minimum(sigma_to, up)
+    return (sigma_to ** 2 - sigma_up ** 2) ** 0.5, sigma_up
+
+
+def lms_coefficients(sigmas, i: int, order: int) -> List[float]:
+    """Linear multistep weights of step i: c_j = integral over [sigma_i, sigma_{i+1}] of the Lagrange basis polynomial through
+    sigma_i, ..., sigma_{i-order+1} that is 1 at sigma_{i-j}.  The integrand has degree order - 1, so Gauss-Legendre quadrature
+    with `order` nodes is exact."""
+    import numpy as np
+    if order - 1 > i:
+        raise ValueError(f"order {order} too high for step {i}")
+    s = [float(v) for v in sigmas]
+    a, b = s[i], s[i + 1]
+    nodes, weights = np.polynomial.legendre.leggauss(max(order, 1))
+    tau = 0.5 * (b - a) * nodes + 0.5 * (a + b)
+    out = []
+    for j in range(order):
+        basis = np.ones_like(tau)
+        for k in range(order):
+            if k != j:
+                basis *= (tau - s[i - k]) / (s[i - j] - s[i - k])
+        out.append(float(0.5 * (b - a) * np.dot(weights, basis)))
+    return out
+
+
+def _lincomb(terms) -> torch.Tensor:
+    """sum_k c_k x_k over any number of (x_k, c_k [F]) terms: hi3d_sampler_lincomb, 8 terms per launch."""
+    out = ops.sampler_lincomb8(torch.empty_like(terms[0][0]), terms[:8])
+    rest = terms[8:]
+    while rest:
+        out = ops.sampler_lincomb8(out, [(out, torch.ones_like(terms[0][1]))] + rest[:7])
+        rest = rest[7:]
+    return out
+
+
+class AncestralSampler(SingleStepDiffusionSampler):
+    """sampling.py:150-187."""
+
+    def __init__(self, eta=1.0, s_noise=1.0, *args, **kwargs):
+        super().__init__(*args, **kwargs)
+        self.eta, self.s_noise = eta, s_noise
+
+    def ancestral_euler_step(self, x, denoised, sigma, sigma_down):
+        return self.euler_step(x, (x - denoised) / append_dims(sigma, x.ndim), append_dims(sigma_down - sigma, x.ndim))
+
+    def ancestral_step(self, x, sigma, next_sigma, sigma_up):
+        noised = x + self.draw_noise(x) * self.s_noise * append_dims(sigma_up, x.ndim)
+        return torch.where(append_dims(next_sigma, x.ndim) > 0.0, noised, x)
+
+    def __call__(self, denoiser, x, cond, uc=None, num_steps=None):
+        x, s_in, sigmas, num_sigmas, cond, uc = self.prepare_sampling_loop(x, cond, uc, num_steps)
+        self._fused_state(denoiser, x, cond, uc, refresh=True)
+        for i in self.get_sigma_gen(num_sigmas):
+            x = self.sampler_step(s_in * sigmas[i], s_in * sigmas[i + 1], denoiser, x, cond, uc)
+        return x
+
+
+class EulerAncestralSampler(AncestralSampler):
+    """sampling.py:254-261: Euler to sigma_down, then noise up to sigma_next; on the fused path one graph replay a step."""
+
+    def sampler_step(self, sigma, next_sigma, denoiser, x, cond, uc=None):
+        sigma_down, sigma_up = ancestral_sigmas(sigma, next_sigma, self.eta)
+        st = self._fused_state(denoiser, x, cond, default(uc, cond), refresh=False)
+        if st is not None:
+            eps = self.draw_noise(x, st.noise_buffer())
+            return st.run(x, sigma, sigma_down, noise=(eps, self.s_noise, sigma_up, next_sigma))[0]
+        denoised = self.denoise(x, denoiser, sigma, cond, uc)
+        x = self.ancestral_euler_step(x, denoised, sigma, sigma_down)
+        return self.ancestral_step(x, sigma, next_sigma, sigma_up)
+
+
+class DPMPP2SAncestralSampler(AncestralSampler):
+    """sampling.py:264-301: DPM-Solver++(2S) to sigma_down (a second evaluation at the log-midpoint), then ancestral noise."""
+
+    def sampler_step(self, sigma, next_sigma, denoiser, x, cond, uc=None, **kwargs):
+        sigma_down, sigma_up = ancestral_sigmas(sigma, next_sigma, self.eta)
+        st = self._fused_state(denoiser, x, cond, default(uc, cond), refresh=False)
+        if st is not None:
+            eps = self.draw_noise(x)
+            x_euler, denoised, _ = st.run(x, sigma, sigma_down, want_denoised=True)
+        else:
+            denoised = self.denoise(x, denoiser, sigma, cond, uc)
+            x_euler = self.ancestral_euler_step(x, denoised, sigma, sigma_down)
+        second = float(sigma_down.sum()) >= 1e-14          # saves the second evaluation when every sigma_down is 0
+        if second:
+            t, t_down = sigma.log().neg(), sigma_down.log().neg()
+            h = t_down - t
+            sigma_mid = (t + 0.5 * h).neg().exp()
+            k_mid, g_mid = sigma_mid / sigma, (-0.5 * h).expm1()
+            k_down, g_down = sigma_down / sigma, (-h).expm1()
+        if st is None:
+            if second:
+                x2 = append_dims(k_mid, x.ndim) * x - append_dims(g_mid, x.ndim) * denoised
+                denoised2 = self.denoise(x2, denoiser, sigma_mid, cond, uc)
+                x_2s = append_dims(k_down, x.ndim) * x - append_dims(g_down, x.ndim) * denoised2
+                x_euler = torch.where(append_dims(sigma_down, x.ndim) > 0.0, x_2s, x_euler)
+            return self.ancestral_step(x_euler, sigma, next_sigma, sigma_up)
+        f32 = lambda v: v.float().contiguous()                                         # noqa: E731
+        noise = f32(self.s_noise * sigma_up * (next_sigma > 0.0))
+        if not second:
+            return _lincomb([(x_euler, f32(torch.ones_like(sigma))), (eps, noise)])
+        x2 = _lincomb([(x, f32(k_mid)), (denoised, f32(-g_mid))])
+        denoised2 = st.denoise(x2, f32(sigma_mid))
+        sel = f32(sigma_down > 0.0)
+        # where(sigma_down > 0, (sigma_down/sigma) x - expm1(-h) D2, x_euler) + s_noise sigma_up eps [sigma_next > 0]
+        return _lincomb([(x, f32(k_down) * sel), (x_euler, 1.0 - sel), (denoised2, -f32(g_down) * sel), (eps, noise)])
+
+
+class LinearMultistepSampler(BaseDiffusionSampler):
+    """sampling.py:190-225: linear multistep of `order` over the slopes d = (x - D)/sigma of the last steps.  On the fused path
+    the slopes are never formed: the update is one launch over the (x, D) pairs of the last `order` steps (8 terms at order 4)."""
+
+    def __init__(self, order=4, *args, **kwargs):
+        super().__init__(*args, **kwargs)
+        self.order = order
+
+    def __call__(self, denoiser, x, cond, uc=None, num_steps=None, **kwargs):
+        x, s_in, sigmas, num_sigmas, cond, uc = self.prepare_sampling_loop(x, cond, uc, num_steps)
+        st = None if kwargs else self._fused_state(denoiser, x, cond, uc, refresh=True)
+        sig = sigmas.detach().cpu().numpy()
+        hist = []                                          # (x_j, D_j, sigma_j) or d_j, newest last
+        for i in self.get_sigma_gen(num_sigmas):
+            sigma = s_in * sigmas[i]
+            coeffs = lms_coefficients(sig, i, min(i + 1, self.order))
+            if st is not None:
+                denoised = st.denoise(x, sigma)
+                hist = (hist + [(x, denoised, float(sig[i]))])[-self.order:]
+                terms = [(x, 1.0)]
+                for c, (xj, dj, sj) in zip(coeffs, reversed(hist)):
+                    terms += [(xj, c / sj), (dj, -c / sj)]
+                terms[1] = (terms[1][0], terms[0][1] + terms[1][1])           # x_i appears twice: one coefficient
+                terms = terms[1:]
+                x = _lincomb([(t, torch.full_like(sigma, w)) for t, w in terms])
+                continue
+            if kwargs:
+                denoised = self.guider(denoiser(*self.guider.prepare_inputs(x, sigma, cond, uc), **kwargs), sigma)
+            else:
+                denoised = self.denoise(x, denoiser, sigma, cond, uc)
+            hist = (hist + [(x - denoised) / append_dims(sigma, x.ndim)])[-self.order:]
+            x = x + sum(c * d for c, d in zip(coeffs, reversed(hist)))
+        return x
+
+
+# ------------------------------------------------------------------------------------------------------------
+# the pipelines' --sampler / --steps / --guidance / --cfg_scale / --s_churn / --eta
+# ------------------------------------------------------------------------------------------------------------
+SAMPLER_CHOICES = {"euler": EulerEDMSampler, "heun": HeunEDMSampler, "dpmpp2m": DPMPP2MSampler,
+                   "euler_ancestral": EulerAncestralSampler, "dpmpp2s_ancestral": DPMPP2SAncestralSampler,
+                   "lms": LinearMultistepSampler}
+GUIDANCE_CHOICES = ("config", "linear", "vanilla", "none")
+
+
+def configure_sampler(base: BaseDiffusionSampler, sampler: str = "config", steps: Optional[int] = None,
+                      guidance: str = "config", cfg_scale: Optional[float] = None, s_churn: Optional[float] = None,
+                      eta: Optional[float] = None, num_frames: Optional[int] = None) -> BaseDiffusionSampler:
+    """The model's sampler with the command line's choices applied; `base` itself when every choice is 'config' / None.
+    The discretisation, the noise range and the guidance scales not overridden are the configuration's."""
+    if sampler == "config" and steps is None and guidance == "config" and cfg_scale is None and s_churn is None and eta is None:
+        return base
+    cls = type(base) if sampler == "config" else SAMPLER_CHOICES[sampler]
+    old = base.guider
+    if guidance == "config":
+        if cfg_scale is not None:
+            raise ValueError("--cfg_scale needs --guidance linear or vanilla")
+        guider = old
+    elif guidance == "none":
+        if cfg_scale is not None:
+            raise ValueError("--guidance none has no scale")
+        guider = IdentityGuider()
+    else:
+        max_scale = cfg_scale if cfg_scale is not None else getattr(old, "max_scale", getattr(old, "scale", None))
+        if not isinstance(max_scale, (int, float)):
+            raise ValueError(f"--guidance {guidance} needs --cfg_scale (the configuration's guider has no scale)")
+        if guidance == "vanilla":
+            guider = VanillaCFG(float(max_scale))
+        else:
+            frames = num_frames if num_frames is not None else getattr(old, "num_frames", None)
+            if frames is None:
+                raise ValueError("--guidance linear needs the number of frames")
+            guider = LinearPredictionGuider(float(max_scale), int(frames), min_scale=getattr(old, "min_scale", 1.0))
+    kw = {}
+    if issubclass(cls, EDMSampler):
+        if eta is not None:
+            raise ValueError(f"--eta applies to the ancestral samplers, not {cls.__name__}")
+        kw = dict(s_churn=getattr(base, "s_churn", 0.0) if s_churn is None else float(s_churn),
+                  s_tmin=getattr(base, "s_tmin", 0.0), s_tmax=getattr(base, "s_tmax", float("inf")),
+                  s_noise=getattr(base, "s_noise", 1.0))
+    elif issubclass(cls, AncestralSampler):
+        if s_churn is not None:
+            raise ValueError(f"--s_churn applies to the EDM samplers (euler, heun), not {cls.__name__}")
+        kw = dict(eta=getattr(base, "eta", 1.0) if eta is None else float(eta), s_noise=getattr(base, "s_noise", 1.0))
+    elif s_churn is not None or eta is not None:
+        raise ValueError(f"--s_churn / --eta do not apply to {cls.__name__}")
+    if cls is LinearMultistepSampler:
+        kw["order"] = getattr(base, "order", 4)
+    out = cls(discretization_config={"target": "torch.nn.Identity"}, num_steps=base.num_steps if steps is None else int(steps),
+              verbose=base.verbose, device=base.device, **kw)
+    out.discretization, out.guider = base.discretization, guider
+    return out

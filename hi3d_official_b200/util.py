@@ -26,6 +26,9 @@ TARGET_ALIASES: Dict[str, str] = {
     "sgm.modules.diffusionmodules.sampling.EulerEDMSampler": "hi3d_official_b200.sampling.EulerEDMSampler",
     "sgm.modules.diffusionmodules.sampling.HeunEDMSampler": "hi3d_official_b200.sampling.HeunEDMSampler",
     "sgm.modules.diffusionmodules.sampling.DPMPP2MSampler": "hi3d_official_b200.sampling.DPMPP2MSampler",
+    "sgm.modules.diffusionmodules.sampling.EulerAncestralSampler": "hi3d_official_b200.sampling.EulerAncestralSampler",
+    "sgm.modules.diffusionmodules.sampling.DPMPP2SAncestralSampler": "hi3d_official_b200.sampling.DPMPP2SAncestralSampler",
+    "sgm.modules.diffusionmodules.sampling.LinearMultistepSampler": "hi3d_official_b200.sampling.LinearMultistepSampler",
     "sgm.models.autoencoder.AutoencoderKL": "hi3d_official_b200.vae.AutoencoderKL",
     "sgm.models.autoencoder.AutoencoderKLModeOnly": "hi3d_official_b200.vae.AutoencoderKLModeOnly",
     # north_star's name for the first stage with the temporal decoder (SURVEY F3: no such class in the reference; its parts are

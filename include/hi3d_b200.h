@@ -299,6 +299,32 @@ int hi3d_sampler_post(const void* net, int net_ld, const float* x, const float* 
 int hi3d_sampler_lincomb4(float* out, const float* x0, const float* x1, const float* x2, const float* x3, const float* c0,
                           const float* c1, const float* c2, const float* c3, int F, int64_t per_sample, void* stream);
 
+/* hi3d_sampler_pre for every guider and for churned EDM steps.  guided = 1: out holds 2F rows, uc half first, as
+ * hi3d_sampler_pre; guided = 0 (IdentityGuider, guiders.py:24-29): F rows of x and concat_c only.  sigma fp32 [F] is the noise
+ * level the network sees.  eps (optional) fp32 NCHW [F, Cx, H, W]: the network sees the churned
+ * x_hat = x + (eps * s_noise) * sqrt(sigma^2 - sigma_from^2) (EDMSampler, sampling.py:94-97; sigma = sigma_hat), which is also
+ * written to x_hat_out (required with eps) for the post step. */
+int hi3d_sampler_pre_ex(const float* x, const float* sigma, const float* sigma_from, const float* eps, float s_noise,
+                        const void* concat_uc, const void* concat_c, int concat_is_fp32, int guided, int F, int Cx, int Cc,
+                        int H, int W, int Cpad, void* out, float* c_noise_out, float* x_hat_out, void* stream);
+
+/* The post step of every guider with an ancestral update (AncestralSampler, sampling.py:158-170; get_ancestral_step gives
+ * sigma_to = sigma_down and sigma_up).  scale fp32 [T] (frame t = f % T): net holds 2F rows, CFG-combined as in
+ * hi3d_sampler_post; scale NULL: net holds F rows (IdentityGuider).  x_out = x + (x - D)/sigma * (sigma_to - sigma), then
+ * + (eps * s_noise) * sigma_up where sigma_next > 0 when eps (fp32 NCHW [F, Cx, H, W]) is given.  denoised_out optional: the
+ * guided D(x, sigma) (DPM-Solver++(2S) extrapolates from it). */
+int hi3d_sampler_post_ancestral(const void* net, int net_ld, const float* x, const float* sigma, const float* sigma_to,
+                                const float* scale, int T, const float* eps, float s_noise, const float* sigma_up,
+                                const float* sigma_next, int F, int Cx, int H, int W, float* x_out, float* denoised_out,
+                                void* stream);
+
+/* out = sum_k c_k[f] * x_k over nterms = 1..8 terms; xs / cs are HOST arrays of nterms device pointers (fp32 tensors of F
+ * samples x per_sample values, coefficients fp32 [F]).  LinearMultistepSampler (sampling.py:190-225) of order 4 is one launch
+ * over (x, D) of the last four steps; DPMPP2SAncestralSampler (sampling.py:279-301) selects its update and adds the ancestral
+ * noise in one launch. */
+int hi3d_sampler_lincomb(float* out, const float* const* xs, const float* const* cs, int nterms, int F, int64_t per_sample,
+                         void* stream);
+
 /* Stage-2 re-noise blend (pipeline_i2v_eval_v02.py:131-132): lat = lat*(1-a) + (init*sigma + z)*a, fp32. */
 int hi3d_renoise_blend(float* lat, const float* init, const float* z, float alpha, float sigma, int64_t n,
                        void* stream);

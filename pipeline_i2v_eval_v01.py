@@ -176,6 +176,36 @@ def add_cli_args(ap, stage):
                     help="operand precision of the denoising UNet's convolutions, projections and feed-forwards: fp8 runs them "
                          "on e4m3 tensor cores, which changes the result (the VAE and the conditioner stay fp16); fp8_attn "
                          "also runs every spatial self-attention core on e4m3 tensor cores, which changes the result again")
+    from hi3d_official_b200.sampling import GUIDANCE_CHOICES, SAMPLER_CHOICES
+    ap.add_argument("--sampler", choices=("config",) + tuple(SAMPLER_CHOICES), default="config",
+                    help="the sampler; 'config' keeps the configuration's" + ("" if stage == 1 else
+                         " (stage 2 re-noises between EDM steps: euler or heun only)"))
+    ap.add_argument("--steps", type=int, default=None, help="sampler steps (default: the configuration's)")
+    ap.add_argument("--guidance", choices=GUIDANCE_CHOICES, default="config",
+                    help="linear: the scale rises from 1 to --cfg_scale over the frames (LinearPredictionGuider); vanilla: "
+                         "--cfg_scale for every frame (VanillaCFG); none: no unconditional evaluation (IdentityGuider), half "
+                         "the network rows")
+    ap.add_argument("--cfg_scale", type=float, default=None,
+                    help="guidance scale of --guidance linear / vanilla (default: the configuration's maximum scale)")
+    ap.add_argument("--s_churn", type=float, default=None, help="EDM churn of euler / heun (default: the configuration's)")
+    ap.add_argument("--eta", type=float, default=None, help="ancestral noise of euler_ancestral / dpmpp2s_ancestral (default 1)")
+
+
+def configure_sampler(model, params, stage):
+    """Applies --sampler, --steps, --guidance, --cfg_scale, --s_churn and --eta to the model's sampler (the configuration's
+    when none is given)."""
+    from hi3d_official_b200.sampling import EDMSampler, configure_sampler as configure
+    if params.steps is not None and params.steps < 1:
+        raise SystemExit(f"--steps must be at least 1, got {params.steps}")
+    try:
+        smp = configure(model.sampler, params.sampler, params.steps, params.guidance, params.cfg_scale, params.s_churn,
+                        params.eta, num_frames=model.num_samples)
+    except ValueError as e:
+        raise SystemExit(str(e))
+    if stage == 2 and not isinstance(smp, EDMSampler):
+        raise SystemExit(f"stage 2 drives the sampler one step at a time between re-noise blends (EDMSampler.step_call), which "
+                         f"only the EDM samplers have: --sampler euler or heun, not {type(smp).__name__}")
+    model.sampler = smp
 
 
 def per_image(values, n, flag):
@@ -243,7 +273,7 @@ def main_batch(params, model, T, h):
                                      [plan["elevations"][i] for i in idx], 1, generators=gens)
         randn = per_object_randn((T, 4, h, h), gens, "cuda")
         with torch.no_grad():
-            frames = model.sample_stage1(c, uc, randn)
+            frames = model.sample_stage1(c, uc, randn, generators=gens)
         for j, (d, s) in enumerate(zip(dirs, seeds)):
             mp4 = save_frames(frames[j * T:(j + 1) * T], os.path.join(d, "first_step"), "first")
             print(f"[hi3d-b200] wrote {T} frames {tuple(frames.shape[1:])} to {mp4} (seed {s})")
@@ -256,6 +286,7 @@ def main():
     if len(params.image_path) > 1:
         batch_plan(params)                                                       # argument errors before the model loads
         model = load_model(params.denoise_config, params.denoise_checkpoint, 1, params.tiny, params.precision)
+        configure_sampler(model, params, 1)
         return main_batch(params, model, model.num_samples, 16 if params.tiny else 64)
     image_path, elevation = params.image_path[0], params.elevation[0]
     towers = params.towers[0] if params.towers else None
@@ -264,6 +295,7 @@ def main():
     seed = random.randint(0, 65535) if params.seed is None else params.seed[0]   # v01:33-34
     torch.manual_seed(seed)
     model = load_model(params.denoise_config, params.denoise_checkpoint, 1, params.tiny, params.precision)
+    configure_sampler(model, params, 1)
     T = model.num_samples                                                        # 16 frames
     h = 16 if params.tiny else 64                                                # 512^2 / 8
     if params.cond:

@@ -18,8 +18,8 @@ import random
 import torch
 import torch.nn.functional as F
 
-from pipeline_i2v_eval_v01 import (add_cli_args, batch_plan, cat_cond, cond_from_towers, load_model, load_towers,
-                                   native_towers_ready, save_frames, synthetic_cond)
+from pipeline_i2v_eval_v01 import (add_cli_args, batch_plan, cat_cond, cond_from_towers, configure_sampler, load_model,
+                                   load_towers, native_towers_ready, save_frames, synthetic_cond)
 
 
 def replace_first_frame(frames, output_dir, size):
@@ -89,7 +89,7 @@ def main_batch(params, model, T, h):
             init_latents = per_object_randn((T, 4, h, h), gens, "cuda")
             noise = posterior_noise(model, T, h, [torch.Generator().manual_seed(s) for s in seeds]).cuda()
             z = model.encode_first_stage(frames.half(), noise=noise)
-            out = model.sample_stage2(c, uc, init_latents, z.float())
+            out = model.sample_stage2(c, uc, init_latents, z.float(), generators=gens)
         for j, (d, s) in enumerate(zip(dirs, seeds)):
             mp4 = save_frames(out[j * T:(j + 1) * T], os.path.join(d, "second_step_video"), "second")
             print(f"[hi3d-b200] wrote {T} frames {tuple(out.shape[1:])} to {mp4} (seed {s})")
@@ -99,9 +99,13 @@ def main():
     ap = argparse.ArgumentParser()
     add_cli_args(ap, 2)
     params = ap.parse_args()
+    if params.sampler not in ("config", "euler", "heun"):
+        raise SystemExit(f"stage 2 drives the sampler one step at a time between re-noise blends (EDMSampler.step_call), which "
+                         f"only the EDM samplers have: --sampler euler or heun, not {params.sampler}")
     if len(params.image_path) > 1:
         batch_plan(params)                                                       # argument errors before the model loads
         model = load_model(params.denoise_config, params.denoise_checkpoint, 2, params.tiny, params.precision)
+        configure_sampler(model, params, 2)
         return main_batch(params, model, model.num_samples, 32 if params.tiny else 128)
     elevation = params.elevation[0]
     towers = params.towers[0] if params.towers else None
@@ -110,6 +114,7 @@ def main():
     seed = random.randint(0, 65535) if params.seed is None else params.seed[0]
     torch.manual_seed(seed)
     model = load_model(params.denoise_config, params.denoise_checkpoint, 2, params.tiny, params.precision)
+    configure_sampler(model, params, 2)
     T = model.num_samples
     h = 32 if params.tiny else 128
     frames = load_first_frames(params.output_dir, T, h, params.synthetic)

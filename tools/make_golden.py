@@ -8,6 +8,7 @@ reference checkout exists:
     python tools/make_golden.py --only-video     # the temporal VideoDecoder fixture
     python tools/make_golden.py --only-oracle    # the fixtures of tests/test_oracle_vs_reference.py
     python tools/make_golden.py --only-cpu-surface   # samplers, conditioner pieces, inference configs
+    python tools/make_golden.py --only-cpu-samplers  # ancestral, LMS and churned EDM samplers (test_samplers_more_cpu.py)
 """
 import os
 import sys
@@ -178,8 +179,28 @@ def cpu_surface_fixtures():
 
 
 @torch.no_grad()
+def cpu_sampler_fixtures():
+    """What tests/test_samplers_more_cpu.py compares against: the reference's ancestral, linear multistep and churned EDM
+    samplers x every guider on the analytic toy denoiser, with the noise injected as that test injects it."""
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import test_samplers_more_cpu as TM
+    R.setup()
+    import sgm.modules.diffusionmodules.sampling as RS
+    out = {}
+    for case, (name, extra) in TM.CASES.items():
+        for guider in TM.GUIDERS:
+            smp = getattr(RS, name)(**TM.sampler_kwargs(guider), **extra)
+            out[f"{case}/{guider}"] = TM.run(smp)
+    torch.save(dict(samplers=out), os.path.join(OUT, "ref_cpu_samplers.pt"))
+    print("cpu sampler fixtures", len(out))
+
+
+@torch.no_grad()
 def main():
     os.makedirs(OUT, exist_ok=True)
+    if "--only-cpu-samplers" in sys.argv:
+        cpu_sampler_fixtures()
+        return
     if "--only-cpu-surface" in sys.argv:
         cpu_surface_fixtures()
         return
@@ -229,6 +250,7 @@ def main():
     video_decoder_fixture()
     oracle_fixtures()
     cpu_surface_fixtures()
+    cpu_sampler_fixtures()
 
 
 if __name__ == "__main__":
