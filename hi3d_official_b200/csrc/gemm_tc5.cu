@@ -11,7 +11,8 @@
 //   TEMPORAL : (tf frames) x (ts pixels), tf*ts = 128 -- the temporal taps shift the frame coordinate of a
 //              [C, HW, T, B] view; clip boundaries zero-fill by OOB.
 // Tiles are ordered n-tile fastest, so that CTAs running together share A rows through L2.  Two schedules share the TMA
-// producer (t5_produce), the row mappings and the epilogue arithmetic (t5_stage, then t5_finish_chunk):
+// producer (t5_produce), the row mappings and the epilogue arithmetic (a register pass into a staging tile, then the GELU
+// family, residual and blend on 16-byte chunks of it):
 //
 // gemm_tc5_kernel -- one CTA per 128 x BN output tile (BN in {64, 128, 192, 256}, chosen per call to cover N with the least
 // padding and wave quantisation over the SMs).  Warp roles (128 + 256 NT threads): warpgroup 0 = TMA producer (one elected
@@ -25,10 +26,12 @@
 // of a CTA's tiles, and two consumer warpgroups take its tiles in turn, each owning a whole 128 x BN tile (BN in {64, 128}) and
 // its own staging tile.  Their MMA turns alternate, so one warpgroup's epilogue runs while the other's main loop has the tensor
 // cores.  With K short the epilogue is as long as the main loop, and the single-tile kernel leaves the tensor cores idle for it.
+// Its epilogue is specialised at compile time (GEGLU, residual / blend) and its staged tiles leave by TMA stores.
 //
-// Selection (tc5_choose, the only place): an fp16 GEMM with K <= 64 T5_PINGPONG_MAX_KT, M >= 128 and at least one tile per SM
-// runs ping-pong; otherwise tile pairs for K >= 1920 with 4 pair tiles per SM, else single tiles.  The hooks
-// hi3d_gemm_tc5_set_pair_mode / set_epilogue_warps force single tiles or pairs, and hi3d_gemm_tc5_schedule reports the choice.
+// Selection (tc5_choose, the only place): an fp16 GEMM with K <= 64 T5_PINGPONG_MAX_KT, M >= 128, at least one tile per SM and
+// not GEGLU together with a residual or blend runs ping-pong; otherwise tile pairs for K >= 1920 with 4 pair tiles per SM, else
+// single tiles.  The hooks hi3d_gemm_tc5_set_pair_mode / set_epilogue_warps force single tiles or pairs, and
+// hi3d_gemm_tc5_schedule reports the choice.
 // The kernels are templated on the operand type: hi3d_gemm_tc5 runs fp16 operands and hi3d_gemm_tc5_fp8 e4m3 ones (wgmma k32,
 // SWIZZLE_64B stages, a per-column weight scale on the fp32 accumulator and an optional e4m3 output).  The e4m3 path keeps the
 // single-tile / pair schedule: its chained accumulation (`part`, see T5_PROMOTE) needs registers beside the accumulator that a
@@ -84,6 +87,7 @@ struct T5Seg {
 struct T5Params {
   CUtensorMap bmap;
   CUtensorMap amap[T5_MAX_MAPS];
+  CUtensorMap omap;   // ping-pong schedule: the output tile's TMA store boxes (see t5_encode_out_map)
   T5Seg seg[HI3D_MAX_SEGS];
   int nseg;
   int M, N, K, mode;
@@ -238,10 +242,8 @@ HI3D_DEVINL void t5_load_chunk(const T5Params& p, long long mo, int nc, Half8& r
   if (p.residual != nullptr) rr = *reinterpret_cast<const Half8*>(p.residual + mo * p.res_ld + nc);
   if (p.blend_x != nullptr) xx = *reinterpret_cast<const Half8*>(p.blend_x + mo * p.blend_ld + nc);
 }
-// The 8 staged halfs v of output row mo, columns nc .. nc + 7, with that chunk's residual rr / blend xx: the GELU family, then
-// the residual add, then the blend; one coalesced store.
-template <bool FP8>
-HI3D_DEVINL void t5_finish_chunk(const T5Params& p, Half8 v, long long mo, int nc, const Half8& rr, const Half8& xx) {
+// Eight staged halfs v with their chunk's residual rr / blend xx: the GELU family, then the residual add, then the blend.
+HI3D_DEVINL void t5_finish_half8(const T5Params& p, Half8& v, const Half8& rr, const Half8& xx) {
   if (p.act >= HI3D_ACT_GELU) store_act_half8(p.act, v);
   if (p.residual != nullptr) {
 #pragma unroll
@@ -258,6 +260,11 @@ HI3D_DEVINL void t5_finish_chunk(const T5Params& p, Half8 v, long long mo, int n
       v.h[q] = __floats2half2_rn(al * b.x + be * a.x, al * b.y + be * a.y);
     }
   }
+}
+// The 8 staged halfs v of output row mo, columns nc .. nc + 7, finished as above; one coalesced store.
+template <bool FP8>
+HI3D_DEVINL void t5_finish_chunk(const T5Params& p, Half8 v, long long mo, int nc, const Half8& rr, const Half8& xx) {
+  t5_finish_half8(p, v, rr, xx);
   if constexpr (FP8) {
     if (p.out_fp8) {
       *reinterpret_cast<uint2*>(reinterpret_cast<uint8_t*>(p.out) + mo * p.out_ld + nc) = half8_to_e4m3(v);
@@ -443,20 +450,117 @@ __global__ void __launch_bounds__(128 + 256 * NT, 1) gemm_tc5_kernel(const __gri
 // parity waits exact: every k-tile a warpgroup waits for is at most one ring lap ahead of the last one consumed.  Each stage is
 // consumed by exactly one warpgroup, so its empty barrier counts that warpgroup's 4 warps.  The k16 MMA sequence of every output
 // element and the epilogue arithmetic are those of gemm_tc5_kernel: results are bit-identical to it.
-constexpr int T5_PP_BATCH = 4;   // ping-pong epilogue: chunks whose global loads are issued together
-template <int BN>
+//
+// The epilogue is specialised on what the UNet's short-K GEMMs ask of it.  GEGLU is a template option, and so is PASS2, the
+// chunk pass that adds the residual and the blend (and applies the GELU family, which follows the fp16 rounding): the register
+// pass then carries no option branch but SiLU and rowbias, which are hoisted out of its unrolled loops.  The warpgroup copies
+// the tile's BN bias values to shared memory once per tile, before the main loop.  The staged tile leaves by TMA stores (p.omap, one 128-row box per 64
+// output columns) issued by one thread of the warpgroup, and is written in the boxes' swizzled layout (T5Stage).
+constexpr int T5_PP_BATCH = 2;   // ping-pong chunk pass: chunks whose global loads are issued together (4 spills at BN = 128)
+
+// The ping-pong staging tile of W fp16 columns: TMA store boxes of BOXC = min(W, 64) columns x 128 rows, one after the other,
+// each row 2 BOXC bytes under the swizzle TMA applies to such rows (SWIZZLE_128B for 128-byte rows, SWIZZLE_64B for 64-byte
+// rows: the 16-byte chunk index is XORed with bits 7.. of the byte offset).  The tile is 1024-byte aligned.
+template <int W>
+struct T5Stage {
+  static constexpr int BOXC = W < 64 ? W : 64, ROWB = 2 * BOXC, BOX_BYTES = T5_BM * ROWB, BOXES = W / BOXC;
+  // byte offset of element (r, c); c even for 4-byte and a multiple of 8 for 16-byte accesses
+  static HI3D_DEVINL uint32_t off(int r, int c) {
+    const uint32_t o = (uint32_t)((c / BOXC) * BOX_BYTES + r * ROWB + (c % BOXC) * 2);
+    return o ^ (((o >> 7) & (ROWB == 128 ? 7u : 3u)) << 4);
+  }
+};
+
+// Register pass of one ping-pong tile (wgmma m64nBN layout, two m64 rows h): accumulator + bias (sbias: the tile's BN bias
+// values, -0 where there is none, as x + -0 = x for every x), rowbias, then SiLU or GEGLU; one fp16 rounding into the staging
+// tile sC.
+template <int BN, bool GEGLU, bool SILU, bool RB>
+HI3D_DEVINL void t5_pp_stage(const T5Params& p, const float (&acc)[2][BN / 2], const float* sbias, uint8_t* sC, int mt,
+                             const T5Tile& o, int n0) {
+  using S = T5Stage<GEGLU ? BN / 2 : BN>;
+  const int lane = threadIdx.x & 31, t4 = lane & 3, warp = (threadIdx.x >> 5) & 3;
+  const int ncols = p.N - n0;   // columns of the tile inside N (rowbias reads stop there)
+#pragma unroll
+  for (int h = 0; h < 2; h++) {
+#pragma unroll
+    for (int hh = 0; hh < 2; hh++) {
+      const int r = h * 64 + warp * 16 + (lane >> 2) + 8 * hh;
+      const __half* rbp = nullptr;
+      if constexpr (RB) {
+        const long long m = t5_row(p, mt, o, r);   // rows past the end (-1) read row 0's rowbias and are not stored
+        rbp = p.rowbias + (long long)(((m < 0 ? 0 : m) / p.rb_div) % p.rb_mod) * p.rb_ld + n0;
+      }
+#pragma unroll
+      for (int j = 0; j < BN / 8; j++) {
+        const int cl = j * 8 + 2 * t4;
+        const float2 b = *reinterpret_cast<const float2*>(sbias + cl);
+        float v0 = acc[h][4 * j + 2 * hh] + b.x, v1 = acc[h][4 * j + 2 * hh + 1] + b.y;
+        if constexpr (RB) {
+          if (j * 8 < ncols) {
+            const __half2 rbv = *reinterpret_cast<const __half2*>(rbp + cl);
+            v0 += __low2float(rbv);
+            v1 += __high2float(rbv);
+          }
+        }
+        if constexpr (GEGLU) {
+          *reinterpret_cast<__half*>(sC + S::off(r, cl >> 1)) = __float2half_rn(v0 * gelu_erf_f(v1));
+        } else {
+          if constexpr (SILU) {
+            v0 = silu_f(v0);
+            v1 = silu_f(v1);
+          }
+          *reinterpret_cast<uint32_t*>(sC + S::off(r, cl)) = pack_half2(v0, v1);
+        }
+      }
+    }
+  }
+}
+
+// Chunk pass of one ping-pong tile (W = BN staged columns): the GELU family, the residual and the blend on the staged tile in
+// place, with coalesced 16-byte residual / blend loads, T5_PP_BATCH chunks per thread in flight.
+template <int W>
+HI3D_DEVINL void t5_pp_pass2(const T5Params& p, uint8_t* sC, int mt, const T5Tile& o, int nout0, int Nout) {
+  using S = T5Stage<W>;
+  constexpr int CPR = W / 8;   // 16-byte chunks per staged row
+  static_assert((T5_BM * CPR) % (128 * T5_PP_BATCH) == 0, "whole batches");
+#pragma unroll 1
+  for (int idx0 = threadIdx.x & 127; idx0 < T5_BM * CPR; idx0 += 128 * T5_PP_BATCH) {
+    long long mo[T5_PP_BATCH];
+    uint32_t so[T5_PP_BATCH];
+    Half8 rr[T5_PP_BATCH], xx[T5_PP_BATCH];
+#pragma unroll
+    for (int u = 0; u < T5_PP_BATCH; u++) {
+      const int idx = idx0 + u * 128, r = idx / CPR, c = (idx % CPR) * 8;
+      so[u] = S::off(r, c);
+      const long long m = nout0 + c < Nout ? t5_row(p, mt, o, r) : -1;
+      mo[u] = m < 0 ? -1 : t5_out_row(p, m);
+      if (mo[u] >= 0) t5_load_chunk(p, mo[u], nout0 + c, rr[u], xx[u]);
+    }
+#pragma unroll
+    for (int u = 0; u < T5_PP_BATCH; u++) {
+      if (mo[u] < 0) continue;
+      Half8 v = *reinterpret_cast<const Half8*>(sC + so[u]);
+      t5_finish_half8(p, v, rr[u], xx[u]);
+      *reinterpret_cast<Half8*>(sC + so[u]) = v;
+    }
+  }
+}
+
+template <int BN, bool GEGLU, bool PASS2>
 __global__ void __launch_bounds__(384, 1) gemm_tc5_pingpong_kernel(const __grid_constant__ T5Params p) {
+  static_assert(!(GEGLU && PASS2), "GEGLU GEMMs with a residual or blend take the single-tile schedule");
   constexpr int ROW = T5Op<__half>::ROW;
   constexpr int A_BYTES = T5_BM * ROW;
   constexpr uint32_t stage_bytes = A_BYTES + BN * ROW;
-  constexpr int pitch = BN + 8;                 // halfs per staged row
+  using S = T5Stage<GEGLU ? BN / 2 : BN>;
+  constexpr uint32_t STAGING_BYTES = T5_BM * BN * sizeof(__half);   // one consumer's staging tile (GEGLU uses half of it)
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;          // SWIZZLE_128B atoms need 1024-byte alignment
   uint8_t* smem = smem_raw + (base - raw);
   const int STAGES = p.stages;
-  __half* const staging = reinterpret_cast<__half*>(smem + STAGES * stage_bytes);   // 2 x 128 x pitch halfs
-  const uint32_t bar_full = base + STAGES * stage_bytes + 2 * T5_BM * pitch * (uint32_t)sizeof(__half);
+  float* const sbias_all = reinterpret_cast<float*>(smem + STAGES * stage_bytes + 2 * STAGING_BYTES);   // 2 x BN floats
+  const uint32_t bar_full = base + STAGES * stage_bytes + 2 * STAGING_BYTES + 2 * BN * (uint32_t)sizeof(float);
   const uint32_t bar_empty = bar_full + 8 * T5Op<__half>::MAX_STAGES;
 
   const int tid = threadIdx.x, lane = tid & 31;
@@ -492,22 +596,25 @@ __global__ void __launch_bounds__(384, 1) gemm_tc5_pingpong_kernel(const __grid_
   // ======================= consumer warpgroups: tiles cw, cw + 2, ... of this CTA =======================
   setmaxnreg_inc<232>();
   const int cw = wg - 1;
-  const int warp = (tid >> 5) & 3;       // warp inside the warpgroup: accumulator rows 16 warp .. + 15 of each m64 row
-  __half* const sC = staging + cw * T5_BM * pitch;
-  const bool geglu = (p.act == HI3D_ACT_GEGLU);
-  const int cpr = (geglu ? BN / 2 : BN) / 8;   // 16-byte chunks per staged row
-  const int Nout = geglu ? p.N / 2 : p.N;
+  const bool leader = (tid & 127) == 0;   // issues and waits for this warpgroup's TMA stores
+  const uint32_t sC_addr = base + STAGES * stage_bytes + cw * STAGING_BYTES;
+  uint8_t* const sC = smem + (sC_addr - base);
+  float* const sbias = sbias_all + cw * BN;
+  const int Nout = GEGLU ? p.N / 2 : p.N;
+  const bool silu = !GEGLU && p.act == HI3D_ACT_SILU;
+  const bool rowbias = p.rowbias != nullptr;
   for (int j = cw; j < n_local; j += 2) {
     const int tile = blockIdx.x + j * gridDim.x;
     const int mt = tile / p.n_tiles, n0 = (tile % p.n_tiles) * BN;
     const T5Tile o = t5_origin(p, mt);
+    // the tile's bias columns, loaded under the main loop (the register pass of tile j - 2 has read them: barrier 4 + cw)
+    for (int c = tid & 127; c < BN; c += 128) sbias[c] = (p.bias != nullptr && n0 + c < p.N) ? __ldg(p.bias + n0 + c) : -0.f;
     float acc[2][BN / 2];
 #pragma unroll
     for (int h = 0; h < 2; h++)
 #pragma unroll
       for (int i = 0; i < BN / 2; i++) acc[h][i] = 0.f;
-    // our MMA turn: the other warpgroup has issued the main loop of tile j - 1 (and, before that, every thread of this
-    // warpgroup has finished reading sC for tile j - 2)
+    // our MMA turn: the other warpgroup has issued the main loop of tile j - 1
     if (j > 0) named_bar_sync(2 + cw, 256);
     uint32_t it = (uint32_t)j * KT;
     uint32_t s = it % STAGES, ph = (it / STAGES) & 1, ps = 0;
@@ -538,48 +645,38 @@ __global__ void __launch_bounds__(384, 1) gemm_tc5_pingpong_kernel(const __grid_
     wgmma_fence_regs(acc[1]);
     if (lane == 0) mbar_arrive(bar_empty + 8 * ps);
 
-    // ---- epilogue phase 1: registers -> (bias, rowbias, activation) -> this warpgroup's fp16 staging tile ----
-#pragma unroll
-    for (int h = 0; h < 2; h++) {
-      const int rl = h * 64 + warp * 16 + (lane >> 2);
-      const long long m[2] = {t5_row(p, mt, o, rl), t5_row(p, mt, o, rl + 8)};
-      t5_stage<BN, false>(p, acc[h], sC, rl, m, n0);
-    }
+    // the TMA stores of this warpgroup's previous tile (issued a whole main loop ago) have read the staging tile, and sbias
+    // is written
+    if (leader && j > cw) bulk_wait_read();
     named_bar_sync(4 + cw, 128);
-
-    // ---- epilogue phase 2: coalesced 16-byte stores with residual / blend ---------------------------
-    const int nout0 = geglu ? n0 / 2 : n0;
-    if (p.residual == nullptr && p.blend_x == nullptr) {
-      for (int idx = tid & 127; idx < T5_BM * cpr; idx += 128) {
-        const int r = idx / cpr, c = idx - r * cpr;
-        const int nc = nout0 + c * 8;
-        if (nc >= Nout) continue;
-        const long long m = t5_row(p, mt, o, r);
-        if (m < 0) continue;
-        t5_store_chunk<false>(p, *reinterpret_cast<const Half8*>(sC + r * pitch + c * 8), m, nc);
-      }
+    // ---- register pass: accumulators -> (bias, rowbias, SiLU / GEGLU) -> staging tile ----
+    if (rowbias) {
+      if (silu) t5_pp_stage<BN, GEGLU, true, true>(p, acc, sbias, sC, mt, o, n0);
+      else t5_pp_stage<BN, GEGLU, false, true>(p, acc, sbias, sC, mt, o, n0);
     } else {
-      // T5_PP_BATCH chunks per thread at a time: their residual / blend loads are all in flight before the first store
-      for (int idx0 = tid & 127; idx0 < T5_BM * cpr; idx0 += 128 * T5_PP_BATCH) {
-        long long mo[T5_PP_BATCH];
-        int nc[T5_PP_BATCH], sofs[T5_PP_BATCH];
-        Half8 rr[T5_PP_BATCH], xx[T5_PP_BATCH];
+      if (silu) t5_pp_stage<BN, GEGLU, true, false>(p, acc, sbias, sC, mt, o, n0);
+      else t5_pp_stage<BN, GEGLU, false, false>(p, acc, sbias, sC, mt, o, n0);
+    }
+    const int nout0 = GEGLU ? n0 / 2 : n0;
+    if constexpr (PASS2) {
+      named_bar_sync(4 + cw, 128);
+      t5_pp_pass2<BN>(p, sC, mt, o, nout0, Nout);
+    }
+    // ---- the staged tile leaves by TMA; rows past M and columns past Nout fall outside the map and are not written ----
+    fence_proxy_async_smem();
+    named_bar_sync(4 + cw, 128);
+    if (leader) {
 #pragma unroll
-        for (int u = 0; u < T5_PP_BATCH; u++) {
-          const int idx = idx0 + u * 128;
-          const int r = idx / cpr, c = idx - r * cpr;
-          nc[u] = nout0 + c * 8;
-          sofs[u] = r * pitch + c * 8;
-          const long long m = (idx < T5_BM * cpr && nc[u] < Nout) ? t5_row(p, mt, o, r) : -1;
-          mo[u] = m < 0 ? -1 : t5_out_row(p, m);
-          if (mo[u] >= 0) t5_load_chunk(p, mo[u], nc[u], rr[u], xx[u]);
-        }
-#pragma unroll
-        for (int u = 0; u < T5_PP_BATCH; u++)
-          if (mo[u] >= 0) t5_finish_chunk<false>(p, *reinterpret_cast<const Half8*>(sC + sofs[u]), mo[u], nc[u], rr[u], xx[u]);
+      for (int b = 0; b < S::BOXES; b++) {
+        const int c0 = nout0 + b * S::BOXC;
+        if (c0 >= Nout) break;
+        if (p.mode == HI3D_ROWS_PLAIN) tma_store_2d(&p.omap, sC_addr + b * S::BOX_BYTES, c0, mt * T5_BM);
+        else tma_store_4d(&p.omap, sC_addr + b * S::BOX_BYTES, c0, o.x0, o.y0, o.z0);
       }
+      bulk_commit();
     }
   }
+  if (leader) bulk_wait();
 }
 
 // ---- host: tensor maps ---------------------------------------------------------------------------------------
@@ -636,12 +733,50 @@ static int launch_tc5(const T5Params& tp, int grid, int smem, cudaStream_t st) {
   return check_launch("hi3d_gemm_tc5");
 }
 
-template <int BN>
+template <int BN, bool GEGLU, bool PASS2>
 static int launch_pingpong(const T5Params& tp, int grid, int smem, cudaStream_t st) {
   static bool attr_done[HI3D_MAX_DEVICES];
-  if (ensure_dyn_smem(gemm_tc5_pingpong_kernel<BN>, smem, attr_done, "hi3d_gemm_tc5")) return -1;
-  gemm_tc5_pingpong_kernel<BN><<<grid, 384, smem, st>>>(tp);
+  if (ensure_dyn_smem(gemm_tc5_pingpong_kernel<BN, GEGLU, PASS2>, smem, attr_done, "hi3d_gemm_tc5")) return -1;
+  gemm_tc5_pingpong_kernel<BN, GEGLU, PASS2><<<grid, 384, smem, st>>>(tp);
   return check_launch("hi3d_gemm_tc5");
+}
+
+// The ping-pong kernels: tile width x epilogue (GEGLU; bias / rowbias / SiLU only; with the chunk pass for residual, blend and
+// the GELU family).  A GEGLU GEMM with a residual or blend does not run ping-pong (tc5_choose).
+static int launch_pingpong(const T5Params& tp, int BN, int grid, int smem, cudaStream_t st) {
+  const bool geglu = tp.act == HI3D_ACT_GEGLU;
+  const bool pass2 = tp.residual != nullptr || tp.blend_x != nullptr || tp.act >= HI3D_ACT_GELU;
+  if (BN == 64) {
+    if (geglu) return launch_pingpong<64, true, false>(tp, grid, smem, st);
+    return pass2 ? launch_pingpong<64, false, true>(tp, grid, smem, st) : launch_pingpong<64, false, false>(tp, grid, smem, st);
+  }
+  if (geglu) return launch_pingpong<128, true, false>(tp, grid, smem, st);
+  return pass2 ? launch_pingpong<128, false, true>(tp, grid, smem, st) : launch_pingpong<128, false, false>(tp, grid, smem, st);
+}
+
+// The ping-pong output map: the output in the geometry of a tile's rows, boxes of W = min(staged tile width, 64) columns x the
+// tile's 128 rows (t5_row's order), swizzled as T5Stage lays the staging tile out.  Its row strides are out_ld, so a column
+// slice of a wider buffer is written in place; a parity-class upsample conv starts at its class's first output row and steps two
+// output columns / rows per tile column / row.
+static int t5_encode_out_map(const hi3d_gemm_params* p, const T5Params& tp, int BN, CUtensorMap* m) {
+  const bool geglu = p->act == HI3D_ACT_GEGLU;
+  const int W = geglu ? BN / 2 : BN;
+  const cuuint32_t boxc = W < 64 ? W : 64;
+  const CUtensorMapSwizzle sw = boxc == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
+  const cuuint64_t nout = (cuuint64_t)(geglu ? p->N / 2 : p->N), ld = (cuuint64_t)p->out_ld * sizeof(__half);
+  if (p->mode == HI3D_ROWS_PLAIN) {
+    cuuint64_t dims[2] = {nout, (cuuint64_t)p->M};
+    cuuint64_t str[1] = {ld};
+    cuuint32_t box[2] = {boxc, (cuuint32_t)T5_BM};
+    return encode_map(m, p->out, 2, dims, str, box, nullptr, sw);
+  }
+  const cuuint64_t Wo = (cuuint64_t)tp.Wo, Ho = (cuuint64_t)tp.Ho, up = p->out_up ? 2 : 1;
+  const __half* o = (const __half*)p->out;
+  if (p->out_up) o += ((long long)p->out_py * 2 * tp.Wo + p->out_px) * p->out_ld;
+  cuuint64_t dims[4] = {nout, Wo, Ho, (cuuint64_t)tp.Nimg};
+  cuuint64_t str[3] = {up * ld, up * up * Wo * ld, up * up * Wo * Ho * ld};
+  cuuint32_t box[4] = {boxc, (cuuint32_t)tp.tw, (cuuint32_t)tp.th, (cuuint32_t)tp.tn};
+  return encode_map(m, o, 4, dims, str, box, nullptr, sw);
 }
 
 // The ping-pong schedule runs fp16 GEMMs of at most T5_PINGPONG_MAX_KT k-tiles (K <= 1280).  Measured with tools/time_gemm.py on
@@ -677,7 +812,8 @@ static T5Choice tc5_choose(const hi3d_gemm_params* p, int m_tiles) {
     return bn;
   };
   const bool forced = g_ew_mode > 0 || g_pair_mode >= 0;
-  if (!FP8 && !forced && p->K / T5_BK <= T5_PINGPONG_MAX_KT && p->M >= T5_BM) {
+  const bool geglu_res = p->act == HI3D_ACT_GEGLU && (p->residual != nullptr || p->blend_x != nullptr);
+  if (!FP8 && !forced && !geglu_res && p->K / T5_BK <= T5_PINGPONG_MAX_KT && p->M >= T5_BM) {
     const int bn = pick_bn(128, m_tiles);
     if ((long long)m_tiles * ((p->N + bn - 1) / bn) >= sm_count) return {T5_SCHED_PINGPONG, bn, 1};
   }
@@ -794,8 +930,8 @@ static int tc5_gemm(const hi3d_gemm_params* p, const float* w_scale, int out_fp8
   const int BN = ch.BN, ntile = ch.ntile;
   const bool pingpong = ch.sched == T5_SCHED_PINGPONG;
   const int stage_bytes = ntile * T5_BM * ROW + BN * ROW;
-  // the ping-pong schedule keeps one staging tile per consumer warpgroup outside the ring
-  const int staging_bytes = pingpong ? 2 * T5_BM * (BN + 8) * (int)sizeof(__half) : 0;
+  // the ping-pong schedule keeps one staging tile and the tile's bias per consumer warpgroup outside the ring
+  const int staging_bytes = pingpong ? 2 * (T5_BM * BN * (int)sizeof(__half) + BN * (int)sizeof(float)) : 0;
   int stages = (T5_SMEM_BUDGET - staging_bytes) / stage_bytes;
   if (stages > MAX_STAGES) stages = MAX_STAGES;
   tp.stages = stages;
@@ -842,8 +978,10 @@ static int tc5_gemm(const hi3d_gemm_params* p, const float* w_scale, int out_fp8
 
   const int smem = stages * stage_bytes + staging_bytes + 16 * MAX_STAGES + 1024;
   if constexpr (!FP8) {
-    if (pingpong)
-      return BN == 64 ? launch_pingpong<64>(tp, (int)grid, smem, st) : launch_pingpong<128>(tp, (int)grid, smem, st);
+    if (pingpong) {
+      if (t5_encode_out_map(p, tp, BN, &tp.omap)) return -1;
+      return launch_pingpong(tp, BN, (int)grid, smem, st);
+    }
   }
   if (ntile == 2)
     return BN == 64 ? launch_tc5<64, 2, Op>(tp, (int)grid, smem, st) : launch_tc5<128, 2, Op>(tp, (int)grid, smem, st);

@@ -59,6 +59,23 @@ HI3D_DEVINL void tma_load_4d(uint32_t dst, const CUtensorMap* map, uint32_t bar,
       "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
+// Shared -> global tile stores, tracked per issuing thread in bulk groups.  The writers of the source tile make their generic-proxy
+// writes visible to the TMA unit (fence_proxy_async_smem, then a barrier) before one thread issues the store; that thread then
+// commits the group, and waits on it before the tile is written again (bulk_wait_read) and before the CTA exits (bulk_wait).
+HI3D_DEVINL void tma_store_2d(const CUtensorMap* map, uint32_t src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];\n" ::"l"(map), "r"(src), "r"(c0),
+               "r"(c1)
+               : "memory");
+}
+HI3D_DEVINL void tma_store_4d(const CUtensorMap* map, uint32_t src, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];\n" ::"l"(map), "r"(src),
+               "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+               : "memory");
+}
+HI3D_DEVINL void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory"); }
+HI3D_DEVINL void bulk_commit() { asm volatile("cp.async.bulk.commit_group;\n" ::: "memory"); }
+HI3D_DEVINL void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;\n" ::: "memory"); }
+HI3D_DEVINL void bulk_wait() { asm volatile("cp.async.bulk.wait_group 0;\n" ::: "memory"); }
 
 // ---- wgmma --------------------------------------------------------------------------------------------------------
 // Shared-memory matrix descriptor, 128-byte swizzle: start >> 4 | LBO >> 4 at bit 16 | SBO >> 4 at bit 32 | layout 1
